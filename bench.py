@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W              # our arm (1 process per GPU; torchrun for N>1)
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU path (oracle port)
+    python bench.py --steps K --dump-outputs DIR                     # + the last timed step's results as DIR/*.npy
 
 One "step" = one full train step (H2D of the batch where applicable, forward, backward, gradient all-reduce
 over NCCL for N>1, stabiliser check, fused SGD) of Cube R-CNN DLA34_FPN on a synthetic batch of 32 images
@@ -46,11 +47,13 @@ def parse():
     ap.add_argument("--skip-iou", action="store_true")
     ap.add_argument("--skip-torch-baseline", action="store_true",
                     help="do not time the oracle model in stock PyTorch eager on the GPU (baseline_torch_gpu)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -89,7 +92,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", 1404.6), d.get("hbm_gbs", 6574.1), "measured (MEASURED_PEAKS.json)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not measured"
 
 
 def _hbm_peak_gbs():
@@ -163,7 +166,7 @@ def run_reference(args):
 
 def torch_gpu_baseline(config_file, batch, size, steps=5, warmup=2):
     """SURVEY 8d 'baseline_torch_gpu': the oracle restatement of the reference graph (fp32 NCHW nn.Modules, per-image
-    Python loops, detectron2 semantics) executed by stock PyTorch eager on this GPU — cuDNN / cuBLAS sm_100 kernels,
+    Python loops, detectron2 semantics) executed by stock PyTorch eager on this GPU — cuDNN / cuBLAS kernels,
     torchvision ROIAlign / NMS — doing forward + backward + SGD on the SAME batch shape.  fp32 (the reference trains in
     fp32, TF32 off) and bf16 autocast.  This is the library path our kernels have to beat on this box."""
     import statistics
@@ -292,7 +295,7 @@ def conv_roofline(trainer, items, peak_tflops, peak_src, conv_fwd_gmac):
                            "GBps": cls["hbm_bound"][2] / (cls["hbm_bound"][0] * 1e-3) / 1e9 if cls["hbm_bound"][0] else 0.0,
                            "frac_of_hbm_peak": (cls["hbm_bound"][2] / (cls["hbm_bound"][0] * 1e-3) / 1e9 / hbm)
                            if cls["hbm_bound"][0] else 0.0}}
-    return {"bound": "tensor", "kernel": "conv_tc_* / conv_halo_* / conv_wgrad_tc_kernel (tcgen05 implicit GEMM, fwd + dgrad + wgrad)",
+    return {"bound": "tensor", "kernel": "conv_tc_* / conv_halo_* / conv_wgrad_tc_kernel (wgmma implicit GEMM, fwd + dgrad + wgrad)",
             "achieved": ach, "peak": peak_tflops, "unit": "TFLOP/s", "frac": ach / peak_tflops, "traffic": _top_kernel_traffic(),
             "peak_source": peak_src + ", bf16 sustained (kernel timed inside a long step)",
             "launches_per_step": len(rec), "conv_ms_per_step": ms, "algorithmic_tflop_per_step": fl / 1e12,
@@ -393,6 +396,25 @@ def iou_block(peak_hbm, peak_src):
     return out
 
 
+def dump_outputs(out_dir, trainer, n_sample=1 << 21):
+    """What the last timed step handed its caller, for comparing two builds output for output: the step's losses
+    (float64, one file per loss) and the updated parameters and momentum (float32) at a fixed, seeded sample of
+    n_sample positions of the flat arena (the whole arena is larger than the 64 MB this dump may take)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    st = trainer.status(wait=True)
+    for k, v in st["losses"].items():
+        np.save(os.path.join(out_dir, "loss_" + k.replace("/", "_") + ".npy"), np.array(v, dtype=np.float64))
+    np.save(os.path.join(out_dir, "total_loss.npy"), np.array(st["total_loss"], dtype=np.float64))
+    total = trainer.flat_p.numel()
+    idx = np.sort(np.random.RandomState(0).choice(total, size=min(n_sample, total), replace=False))
+    sel = torch.from_numpy(idx).to(trainer.flat_p.device)
+    np.save(os.path.join(out_dir, "params_sample.npy"), trainer.flat_p[sel].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "momentum_sample.npy"), trainer.flat_m[sel].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "sample_index.npy"), idx.astype(np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -453,6 +475,8 @@ def run_ours(args):
         sampler.start()
     ms, launches = timed(resident, args.steps, read_loss=False)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer)
     for i in range(2):
         trainer.step(host[i % 2])
     ms_e2e, _ = timed(host, args.steps, read_loss=True)
@@ -475,7 +499,7 @@ def run_ours(args):
         "config": {"workload": f"Cube R-CNN {C['name']} train step, batch {B}/GPU synthetic {S}x{S}, K=50, G=8 GT/img "
                                f"(BASELINE {C['baseline_cfg']}; weak scaling, global batch {B * world})",
                    "parallelism": f"dp{world}", "l2": "two alternating input batches (39 MB uint8 images each) + ~10 GB of "
-                                                      "activations per step: working set >> 126 MB L2",
+                                                      "activations per step: working set >> 50 MB L2",
                    "cuda_graph": bool(trainer.graph is not None),
                    "images": "uint8 (3,H,W), as cubercnn/data/dataset_mapper.py:35 emits them",
                    "train_gflop_per_image": C["train_gflop"]},

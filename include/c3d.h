@@ -1,5 +1,5 @@
 /*
- * c3d.h — C ABI of libc3d.so, the B200-native (sm_100a) kernels behind the Cube R-CNN hot path.
+ * c3d.h — C ABI of libc3d.so, the H100-native (sm_90a) kernels behind the Cube R-CNN hot path.
  *
  * The reference (facebookresearch/omni3d) is pure Python and has no FFI of its own; every entry
  * point below replaces the third-party native op the reference reaches at the cited call site.
@@ -7,7 +7,10 @@
  * Conventions (all entry points):
  *   - plain pointers + sizes; every pointer is DEVICE memory unless the name ends in _host;
  *   - the caller owns every buffer including the workspace (size from the matching
- *     *_workspace_bytes query); kernels never allocate, free or synchronise;
+ *     *_workspace_bytes query); kernels never allocate, free or synchronise.  The one exception are the weight
+ *     gradients (conv / linear wgrad) split over several CTAs: their per-split partial sums live in scratch from the
+ *     stream-ordered allocator (cudaMallocAsync / cudaFreeAsync on `stream`, which graph capture records) and are
+ *     added in split order, so the gradient is the same on every run;
  *   - work is enqueued on `stream` (a cudaStream_t / CUstream handle passed as void*);
  *   - return 0 (C3D_OK) or a negative c3d_status; c3d_last_error() gives a thread-local string.
  */
@@ -74,7 +77,7 @@ int32_t c3d_box3d_overlap_segmented(const float* boxes_dt, int64_t n_dt, const f
                                     float* iou, int32_t* n_bad, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * NHWC bf16 implicit-GEMM convolution on tcgen05 tensor cores (TMA-staged, fp32 accumulate in TMEM).
+ * NHWC bf16 implicit-GEMM convolution on wgmma tensor cores (TMA-staged, fp32 accumulate in registers).
  * Replaces the cuDNN calls behind nn.Conv2d in cubercnn/modeling/backbone/dla.py:43-51,159-161,
  * 211-214,241-243,287-297, the detectron2 FPN convs built at dla.py:500-506 / resnet.py:88-95 and
  * the StandardRPNHead convs (configs/Base.yaml:49).  Data-gradient = the same entry point with
@@ -116,7 +119,10 @@ int32_t c3d_conv2d_fwd(const c3d_conv_desc* d, const void* x, const void* w, con
 
 /* dw[Cout][KH][KW][Cin] (fp32) += the weight gradient of the convolution described by d, from the
  * forward input x (N,H,W,Cin) and the output gradient dy (N,Ho,Wo,Cout), both bf16 NHWC.
- * Split-K over pixels with fp32 atomics: the caller zeroes (or pre-loads) dw. */
+ * Split-K over pixels, partials summed in a fixed order: the caller zeroes (or pre-loads) dw.
+ * Cin and Cout must be multiples of 16, except for the stride-1 thin-channel layers with (KH, Cin) in
+ * {(7, 8), (3, 16), (3, 32)} and Cout 16 or 32 (same padding, W >= 128 unless Cin = 8), which run on the
+ * rolling-halo kernel; other Cin = 8 layers return C3D_EINVAL. */
 int32_t c3d_conv2d_wgrad(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, void* stream);
 /* same, oihw != 0: dw is the fp32 master-layout gradient [Cout][Cin][KH][KW] (accumulate straight into the
  * optimizer's gradient arena, no layout conversion pass) */
@@ -138,7 +144,7 @@ typedef struct {
 int32_t c3d_pack_conv_weights_batched(const void* descs_dev, int32_t n, int64_t total_elems, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Fully-connected layers on the same tcgen05 kernels (bf16 operands, fp32 accumulate in TMEM, bias + ReLU fused).
+ * Fully-connected layers on the same wgmma kernels (bf16 operands, fp32 accumulate in registers, bias + ReLU fused).
  * Replace the cuBLAS GEMMs behind nn.Linear in detectron2 FastRCNNConvFCHead / FastRCNNOutputLayers
  * (configs/Base.yaml:67-70, cubercnn/modeling/roi_heads/fast_rcnn.py:119-143) and in CubeHead
  * (cubercnn/modeling/roi_heads/cube_head.py:63-73,108-144,146-197).
@@ -146,7 +152,7 @@ int32_t c3d_pack_conv_weights_batched(const void* descs_dev, int32_t n, int64_t 
  *   K % 16 == 0, N % 16 == 0 (callers zero-pad the predictors).
  * c3d_pack_linear_weight: fp32 master (N, K) -> bf16 w (N, K') and (optional) wt (K', N).  C * PP == K with PP > 1
  *   re-orders the input features from (c, p) [NCHW-flattened RoI, the reference's layout] to (p, c) [NHWC-flattened RoI].
- * c3d_linear_wgrad: dw (fp32, += with atomics) = dy^T x.  master_chw != 0: dw is addressed in the master's (c, p)
+ * c3d_linear_wgrad: dw (fp32, +=) = dy^T x.  master_chw != 0: dw is addressed in the master's (c, p)
  *   feature order (accumulate straight into the optimizer's gradient arena), else in the packed (p, c) order.
  * ------------------------------------------------------------------------------------------ */
 int32_t c3d_pack_linear_weight(const float* w, int32_t N, int32_t K, int32_t C, int32_t PP, void* w_bf16, void* wt_bf16,
@@ -253,11 +259,11 @@ int32_t c3d_sgd_momentum_dev(float* p, const float* g, float* mom, int64_t n, co
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
   const void* feat[5];   /* level l: bf16 (N,H[l],W[l],C) */
-  void* grad[5];         /* backward only: fp32 (N,H[l],W[l],C), accumulated with atomics */
+  void* grad[5];         /* backward only: fp32 (N,H[l],W[l],C), += (each element in one fixed order) */
   int32_t H[5], W[5];
   float scale[5];
   int32_t num_levels;
-  int32_t num_images;    /* N of the maps (0 = do not check the image index) */
+  int32_t num_images;    /* N of the maps (0 = do not check the image index; c3d_roi_align_bwd requires it) */
 } c3d_roi_levels;
 int32_t c3d_roi_align_fwd(const c3d_roi_levels* levels, const float* rois, int32_t R, int32_t C, int32_t pooled_h,
                           int32_t pooled_w, void* out, void* stream);

@@ -1,4 +1,4 @@
-"""omni3d_b200 — B200-native (sm_100a) Cube R-CNN hot path behind the reference's interface.
+"""omni3d_b200 — H100-native (sm_90a) Cube R-CNN hot path behind the reference's interface.
 
 Product code.  Never imports oracle/.  Every op fails loudly if libc3d.so (the hand-written
 CUDA kernels, C ABI in include/c3d.h) is missing — there is no CPU or library fallback.

@@ -3,7 +3,7 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# C3D_LIB_PATH: developer override (the lab build libc3d_lab.so of csrc/Makefile `make lab`); never a fallback
+# C3D_LIB_PATH: developer override (an alternative build of the library); never a fallback
 LIB_PATH = os.environ.get("C3D_LIB_PATH") or os.path.join(_HERE, "libc3d.so")
 _lib = None
 

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's 3D-IoU interface, running on libc3d.so (sm_100a).
+"""Host-side mirror of the reference's 3D-IoU interface, running on libc3d.so (sm_90a).
 
     box3d_overlap(boxes_dt, boxes_gt, eps_coplanar=1e-4, eps_nonzero=1e-8) -> iou (N, M)
         == cubercnn/evaluation/omni3d_evaluation.py:106-166 (same name, argument meaning and

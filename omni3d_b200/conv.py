@@ -1,4 +1,4 @@
-"""ctypes front-end of the tcgen05 implicit-GEMM convolution entry points (include/c3d.h).
+"""ctypes front-end of the wgmma implicit-GEMM convolution entry points (include/c3d.h).
 
 Tensors are torch CUDA tensors used as raw device buffers: activations NHWC bf16 (N,H,W,C),
 weights OHWI bf16 (Cout,KH,KW,Cin).  No torch types cross the ABI.

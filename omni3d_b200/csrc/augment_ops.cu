@@ -49,7 +49,7 @@ extern "C" int32_t c3d_resize_bilinear_u8(const uint8_t* img_hwc, int32_t H, int
       new_w < 1 || ksize_h < 1 || ksize_v < 1 || row_first < 0 || row_last > H || row_first >= row_last)
     return set_error(C3D_EINVAL, "resize_bilinear_u8: bad args");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  auto blocks = [](long long n) { long long b = (n + 255) / 256; return (unsigned)(b > 148 * 16 ? 148 * 16 : (b < 1 ? 1 : b)); };
+  auto blocks = [](long long n) { long long b = (n + 255) / 256; return (unsigned)(b > kNumSMs * 16 ? kNumSMs * 16 : (b < 1 ? 1 : b)); };
   // pass 1 (horizontal): img (H,W,C) -> tmp (H,new_w,C), only the rows the vertical pass reads
   resample_u8_kernel<<<blocks((long long)(row_last - row_first) * new_w * C), 256, 0, st>>>(
       img_hwc, C, (long long)W * C, 1, tmp_hwc, C, (long long)new_w * C, 1, new_w, row_first, row_last, H, C, bounds_h, kk_h,

@@ -1,4 +1,4 @@
-// box3d_geom.cuh — per-lane geometry of the oriented-box 3D IoU (sm_100a device code; the
+// box3d_geom.cuh — per-lane geometry of the oriented-box 3D IoU (sm_90a device code; the
 // functions are __host__ __device__ so tests/csrc/geom_host_harness.cpp can run them on the
 // CPU and compare bit-for-bit with the oracle without a GPU).
 //

@@ -1,4 +1,4 @@
-// box3d_overlap.cu — oriented-box 3D IoU for B200 (sm_100a).  Compile with -fmad=false.
+// box3d_overlap.cu — oriented-box 3D IoU for H100 (sm_90a).  Compile with -fmad=false.
 //
 // Replaces pytorch3d._C.iou_box3d (cubercnn/evaluation/omni3d_evaluation.py:155) and the
 // reference wrapper box3d_overlap (omni3d_evaluation.py:106-166).

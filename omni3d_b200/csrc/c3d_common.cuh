@@ -12,5 +12,5 @@ inline int32_t check_launch(const char* what) {
   if (e != cudaSuccess) return set_error(C3D_ECUDA, "%s: %s", what, cudaGetErrorString(e));
   return C3D_OK;
 }
-constexpr int kNumSMs = 148;     // B200
+constexpr int kNumSMs = 132;     // H100 SXM
 }  // namespace c3d

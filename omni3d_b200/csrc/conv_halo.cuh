@@ -1,21 +1,21 @@
-// conv_halo.cuh — "thin-channel" stride-1 convolutions (Cin, Cout <= 32) on tcgen05 with a rolling halo of input
+// conv_halo.cuh — "thin-channel" stride-1 convolutions (Cin, Cout <= 32) on wgmma with a rolling halo of input
 // rows in shared memory.  Included by conv_tc.cu (same translation unit: shares the tensor-map encoder).
 //
 // Why a second kernel: for the 640x640 stem (7x7, 3->16) and level0 (3x3, 16->16) of DLA-34
 // (cubercnn/modeling/backbone/dla.py:287-297) the tap-per-TMA-box implicit GEMM of conv_tc_kernel moves
 // taps x 128 px x Cin x 2 B through L2->smem per 128 output pixels (196 KB for the stem) while the math is tiny:
-// the layer is L2->SM bandwidth bound at ~20x its HBM roofline.  Here every input row is brought to shared memory
-// ONCE per 128-pixel strip, as planes of 8 channels ([plane][pixel][8 ch], 16 B per pixel), and the tensor core
-// reads its A operand *in place* through no-swizzle (INTERLEAVE) UMMA descriptors:
-//   K-major canonical form  ((8,m),(T,2)) : ((16 B, SBO), (1, LBO))        (cute/atom/mma_traits_sm100.hpp:192-197)
+// the layer would be L2->SM bandwidth bound far above its HBM roofline.  Here every input row is brought to shared
+// memory ONCE per 128-pixel strip, as planes of 8 channels ([plane][pixel][8 ch], 16 B per pixel), and the tensor
+// core reads its A operand *in place* through no-swizzle (INTERLEAVE) wgmma descriptors:
+//   K-major canonical form  ((8,m),(T,2)) : ((16 B, SBO), (1, LBO))        (cute GMMA::Layout_K_INTER_Atom)
 //   rows = consecutive pixels (16 B apart, SBO = 128 B per group of 8), the two 8-wide K chunks of one MMA are
 //   either two channel planes (LBO = plane bytes) or — for the 8-channel stem — two adjacent taps (LBO = 16 B).
 // A filter tap is therefore just a different descriptor start address (+kw*16 B, other ring slot for kh): no
 // im2col copy exists anywhere.  The CTA walks down a strip, so each new output row costs ONE new input row of TMA.
 //
-// The weight gradient uses the same resident rows as an MN-major operand: M = 16 pixel shifts (= kw) x 8 channels,
-// K = pixels, N = Cout from dY staged the same way; one TMEM block per (kh, plane) accumulates over every row the
-// CTA visits and is flushed once with fp32 atomics.
+// The weight gradient uses the same resident rows as an MN-major operand: M = 8 pixel shifts (= kw) x 8 channels,
+// K = pixels, N = Cout from dY staged the same way; one register accumulator per (kh, plane) accumulates over every
+// row the CTA visits and is stored once as the CTA's partial; the partials are summed in CTA order.
 #pragma once
 
 namespace c3d {
@@ -38,25 +38,25 @@ struct HaloParams {
   int PO;                     // output channel planes (Cout / 8)
   int RD;                     // dY ring slots
   float* dw;
+  float* part;                // per-CTA partials [gridDim.x][welems], summed in CTA order (null: a single CTA adds into dw)
+  long long welems;
   int oihw;
 };
 
+// descriptor halves: lo = start>>4 | (LBO>>4)<<16, hi = SBO>>4 | layout none (interleave)
+__device__ __forceinline__ uint64_t halo_desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | (uint64_t)lo; }
+__host__ __device__ constexpr uint32_t halo_desc_hi(uint32_t sbo_bytes) { return (sbo_bytes >> 4) & 0x3FFFu; }
+
 // ------------------------------------------------------------------------------------------------------------
 // forward / data-gradient: y[n,y,x,:] = sum_taps W[:,kh,kw,:] . x[n, y+kh-pad, x+kw-pad, :]
-// warp 0 = TMA producer, warp 1 = MMA issuer, warps 2-5 = epilogue.  CH = Cout / 16 (1 or 2).
-// descriptor halves: lo = start>>4 | (LBO>>4)<<16, hi = SBO>>4 | version 1 (bit 46) | layout none
-__device__ __forceinline__ uint64_t halo_desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | (uint64_t)lo; }
-__host__ __device__ constexpr uint32_t halo_desc_hi(uint32_t sbo_bytes) { return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14); }
-
-// KS / CIN > 0 fix the filter size and input channels at compile time: the MMA-issuing thread is a single lane whose
-// instruction latency bounds the kernel (measured: ~6 cycles per dependent instruction), so its per-MMA address
-// arithmetic must fold to immediates.  KS = CIN = 0 is the generic (slow) fallback.
+// warp 8 = TMA producer; warps 0-7 = two consumer warpgroups, pixels 0..63 / 64..127 of the strip row (M = 64 each).
+// CH = Cout / 16 (1 or 2).
+// KS / CIN > 0 fix the filter size and input channels at compile time so that the per-MMA descriptor arithmetic folds
+// to immediates.  KS = CIN = 0 is the generic (slow) fallback.
 template <int CH, int KS, int CIN>
-__global__ void __launch_bounds__(192, CH == 1 ? 3 : 2)
+__global__ void __launch_bounds__(kGemmThreads, CH == 1 ? 3 : 2)
 conv_halo_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const HaloParams P) {
   constexpr int kCout = CH * 16;
-  constexpr int kAcc = 4;                                         // TMEM accumulator ring (rows in flight MMA -> epilogue)
-  constexpr uint32_t kTmemCols = 128;
   const int KH = KS > 0 ? KS : P.KH, KW = KH;
   const int Cin = CIN > 0 ? CIN : P.Cin;
   const int BW = KS > 1 ? 136 : P.BW;
@@ -70,10 +70,7 @@ conv_halo_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const HaloParam
   uint8_t* ring = smem + ((wimg_bytes + 127) & ~127);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ring + (size_t)P.R * slot_bytes);
   uint64_t* empty_bar = full_bar + P.R;
-  uint64_t* tfull_bar = empty_bar + P.R;
-  uint64_t* tempty_bar = tfull_bar + kAcc;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty_bar + kAcc);
-  float* red = reinterpret_cast<float*>(tmem_ptr + 4);            // [4 warps][2][kCout]
+  float* red = reinterpret_cast<float*>(empty_bar + P.R);         // [8 warps][2][kCout]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int KWP = (KW + 1) >> 1;                                  // tap pairs per filter row (Cin == 8 mode)
@@ -95,19 +92,14 @@ conv_halo_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const HaloParam
   }
   ptx::fence_proxy_async();
 
-  if (warp == 0 && lane == 0) ptx::prefetch_tensormap(&tmap_x);
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < P.R; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < kAcc; ++a) { ptx::mbar_init(&tfull_bar[a], 1); ptx::mbar_init(&tempty_bar[a], 4); }
+  if (warp == kConsumerWarps && lane == 0) {
+    ptx::prefetch_tensormap(&tmap_x);
+    for (int s = 0; s < P.R; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kConsumerWarps); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) ptx::tmem_alloc<kTmemCols>(tmem_ptr);
-  ptx::tcgen05_fence_before();
   __syncthreads();
-  ptx::tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     if (ptx::elect_one()) {
       uint32_t slot = 0, par = 0;
       for (int c = blockIdx.x; c < P.total_chunks; c += gridDim.x) {
@@ -127,213 +119,161 @@ conv_halo_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const HaloParam
         }
       }
     }
-  } else if (warp == 1) {
-    if (ptx::elect_one()) {
-      const uint32_t idesc = ptx::make_idesc_bf16(128, kCout, 0, 0);
-      const uint32_t R = (uint32_t)P.R;
-      const uint32_t slot_u = (uint32_t)slot_bytes >> 4;                         // descriptor address units (16 B)
-      const uint32_t a_lo0 = (ptx::smem_u32(ring) >> 4) | ((pair_mode ? 1u : ((uint32_t)plane_bytes >> 4)) << 16);
-      const uint32_t b_lo0 = (ptx::smem_u32(wimg) >> 4) | (8u << 16);           // LBO 128 B
-      constexpr uint32_t a_hi = halo_desc_hi(128), b_hi = halo_desc_hi(256);
-      uint32_t slot0 = 0;                      // ring slot of the first input row of the current output row
-      uint32_t rslot = 0, rpar = 0;            // next ring slot to wait for
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int c = blockIdx.x; c < P.total_chunks; c += gridDim.x) {
-        const int cy = c % P.chunks_per_col;
-        const int y0 = cy * P.rows_per_chunk;
-        const int rows = min(P.rows_per_chunk, P.H - y0);
-        for (int j = 0; j < rows; ++j) {
-          const int need = j == 0 ? KH : 1;
-          for (int t = 0; t < need; ++t) {
-            ptx::mbar_wait(&full_bar[rslot], rpar);
-            if (++rslot == R) { rslot = 0; rpar ^= 1u; }
-          }
-          ptx::mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-          ptx::tcgen05_fence_after();
-          const uint32_t tacc = tmem_base + (uint32_t)acc * kCout;
-          uint32_t sl = slot0;
-          int s = 0;
-#pragma unroll
-          for (int kh = 0; kh < KH; ++kh) {
-            const uint32_t row_lo = a_lo0 + sl * slot_u;
-            if (pair_mode) {
-#pragma unroll
-              for (int pp = 0; pp < KWP; ++pp, ++s)
-                ptx::umma_bf16(tacc, halo_desc(row_lo + (uint32_t)(2 * pp), a_hi),
-                               halo_desc(b_lo0 + (uint32_t)(s * kCout * 2), b_hi), idesc, s != 0 ? 1u : 0u);
-            } else {
-#pragma unroll
-              for (int kw = 0; kw < KW; ++kw)
-#pragma unroll
-                for (int q = 0; q < PQ; ++q, ++s)
-                  ptx::umma_bf16(tacc, halo_desc(row_lo + (uint32_t)(2 * q) * ((uint32_t)plane_bytes >> 4) + (uint32_t)kw, a_hi),
-                                 halo_desc(b_lo0 + (uint32_t)(s * kCout * 2), b_hi), idesc, s != 0 ? 1u : 0u);
-            }
-            if (++sl == R) sl = 0;
-          }
-          ptx::umma_commit(&empty_bar[slot0]);                   // the oldest row of the window is no longer needed
-          ptx::umma_commit(&tfull_bar[acc]);
-          if (++slot0 == R) slot0 = 0;
-          if (++acc == kAcc) { acc = 0; acc_phase ^= 1u; }
-        }
-        for (int t = 0; t < KH - 1; ++t) {                       // rows only the finished chunk used
-          ptx::umma_commit(&empty_bar[slot0]);
-          if (++slot0 == R) slot0 = 0;
-        }
-      }
-    }
   } else {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    int acc = 0; uint32_t acc_phase = 0;
-    float s1[kCout], s2[kCout];
+    const uint32_t R = (uint32_t)P.R;
+    const uint32_t slot_u = (uint32_t)slot_bytes >> 4;                         // descriptor address units (16 B)
+    // A: this warpgroup's 64 pixels start 64 x 16 B into the row
+    const uint32_t a_lo0 = ((ptx::smem_u32(ring) >> 4) + (uint32_t)((warp >> 2) * 64)) |
+                           ((pair_mode ? 1u : ((uint32_t)plane_bytes >> 4)) << 16);
+    const uint32_t b_lo0 = (ptx::smem_u32(wimg) >> 4) | (8u << 16);           // LBO 128 B
+    constexpr uint32_t a_hi = halo_desc_hi(128), b_hi = halo_desc_hi(256);
+    const int cq = 2 * (lane & 3);
+    uint32_t slot0 = 0;                      // ring slot of the first input row of the current output row
+    uint32_t rslot = 0, rpar = 0;            // next ring slot to wait for
+    float s1[4 * CH], s2[4 * CH];            // statistics of this thread's channels (8j + cq, +1)
 #pragma unroll
-    for (int i = 0; i < kCout; ++i) { s1[i] = 0.f; s2[i] = 0.f; }
+    for (int i = 0; i < 4 * CH; ++i) { s1[i] = 0.f; s2[i] = 0.f; }
     for (int c = blockIdx.x; c < P.total_chunks; c += gridDim.x) {
       const int col = c / P.chunks_per_col, cy = c - col * P.chunks_per_col;
       const int n = col / P.strips, xs = col - n * P.strips;
       const int y0 = cy * P.rows_per_chunk;
       const int rows = min(P.rows_per_chunk, P.H - y0);
-      const int x = xs * 128 + m;
-      const bool valid = x < P.W;
+      int xh[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) xh[h] = xs * 128 + (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
       for (int j = 0; j < rows; ++j) {
-        const long long pix = (long long)n * P.out_img_stride + (long long)(y0 + j) * P.out_h_stride +
-                              (long long)x * P.out_w_stride + P.out_off;
-        ptx::mbar_wait(&tfull_bar[acc], acc_phase);
-        ptx::tcgen05_fence_after();
-        const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * kCout;
-        uint32_t v[CH][16];
+        const int need = j == 0 ? KH : 1;
+        for (int t = 0; t < need; ++t) {
+          ptx::mbar_wait(&full_bar[rslot], rpar);
+          if (++rslot == R) { rslot = 0; rpar ^= 1u; }
+        }
+        float acc[kCout / 2];
+        uint32_t sl = slot0;
+        int s = 0;
+        ptx::wgmma_fence();
 #pragma unroll
-        for (int ch = 0; ch < CH; ++ch) ptx::tmem_ld_32x32b_x16(tacc + (uint32_t)(ch * 16), v[ch]);
-        ptx::tmem_ld_wait();
-        // accumulator is in registers: hand the TMEM buffer back before the stores
-        ptx::tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tempty_bar[acc]);
-        if (++acc == kAcc) { acc = 0; acc_phase ^= 1u; }
+        for (int kh = 0; kh < KH; ++kh) {
+          const uint32_t row_lo = a_lo0 + sl * slot_u;
+          if (pair_mode) {
 #pragma unroll
-        for (int ch = 0; ch < CH; ++ch) {
-          float f[16];
+            for (int pp = 0; pp < KWP; ++pp, ++s)
+              ptx::wgmma_bf16<kCout, 0, 0>(acc, halo_desc(row_lo + (uint32_t)(2 * pp), a_hi),
+                                            halo_desc(b_lo0 + (uint32_t)(s * kCout * 2), b_hi), s != 0 ? 1u : 0u);
+          } else {
 #pragma unroll
-          for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[ch][i]);
-          if (P.stats) {
+            for (int kw = 0; kw < KW; ++kw)
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float xv = valid ? f[i] : 0.f;
-              s1[ch * 16 + i] += xv;
-              s2[ch * 16 + i] += xv * xv;
-            }
+              for (int q = 0; q < PQ; ++q, ++s)
+                ptx::wgmma_bf16<kCout, 0, 0>(acc, halo_desc(row_lo + (uint32_t)(2 * q) * ((uint32_t)plane_bytes >> 4) + (uint32_t)kw, a_hi),
+                                              halo_desc(b_lo0 + (uint32_t)(s * kCout * 2), b_hi), s != 0 ? 1u : 0u);
           }
-          if (valid) {
-            const int c0 = ch * 16;
-            if (P.bias) {
+          if (++sl == R) sl = 0;
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(acc);
+        // the oldest row of the window is no longer needed
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[slot0]);
+        if (++slot0 == R) slot0 = 0;
 #pragma unroll
-              for (int i = 0; i < 16; ++i) f[i] += __ldg(P.bias + c0 + i);
+        for (int h = 0; h < 2; ++h) {
+          if (xh[h] >= P.W) continue;
+          const long long pix = (long long)n * P.out_img_stride + (long long)(y0 + j) * P.out_h_stride +
+                                (long long)xh[h] * P.out_w_stride + P.out_off;
+#pragma unroll
+          for (int jb = 0; jb < 2 * CH; ++jb) {
+            const int c0 = 8 * jb + cq;
+            float v0 = acc[4 * jb + 2 * h], v1 = acc[4 * jb + 2 * h + 1];
+            if (P.stats) {
+              s1[2 * jb] += v0; s1[2 * jb + 1] += v1;
+              s2[2 * jb] += v0 * v0; s2[2 * jb + 1] += v1 * v1;
             }
-            if (P.relu) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) f[i] = fmaxf(f[i], 0.f);
-            }
-            if (P.out_fp32) {
-              float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(P.out) + pix * P.out_pix_stride + c0);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) op[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-            } else {
-              uint32_t pk[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                __nv_bfloat162 h = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-                pk[i] = *reinterpret_cast<uint32_t*>(&h);
-              }
-              uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(P.out) + pix * P.out_pix_stride + c0);
-              op[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-              op[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-            }
+            if (P.bias) { v0 += __ldg(P.bias + c0); v1 += __ldg(P.bias + c0 + 1); }
+            if (P.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (P.out_fp32)
+              *reinterpret_cast<float2*>(reinterpret_cast<float*>(P.out) + pix * P.out_pix_stride + c0) = make_float2(v0, v1);
+            else
+              *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(P.out) + pix * P.out_pix_stride + c0) =
+                  __floats2bfloat162_rn(v0, v1);
           }
         }
+      }
+      for (int t = 0; t < KH - 1; ++t) {                         // rows only the finished chunk used
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[slot0]);
+        if (++slot0 == R) slot0 = 0;
       }
     }
     if (P.stats) {          // one partial-statistics row per CTA (BatchNorm batch statistics, fp32 partials)
 #pragma unroll
-      for (int i = 0; i < kCout; ++i) {
+      for (int i = 0; i < 4 * CH; ++i) {
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
+        for (int o = 4; o < 32; o <<= 1) {
           s1[i] += __shfl_xor_sync(0xffffffffu, s1[i], o);
           s2[i] += __shfl_xor_sync(0xffffffffu, s2[i], o);
         }
       }
-      if (lane == 0) {
+      if (lane < 4) {
 #pragma unroll
-        for (int i = 0; i < kCout; ++i) { red[(q * 2 + 0) * kCout + i] = s1[i]; red[(q * 2 + 1) * kCout + i] = s2[i]; }
+        for (int jb = 0; jb < 2 * CH; ++jb)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            red[(warp * 2 + 0) * kCout + 8 * jb + cq + e] = s1[2 * jb + e];
+            red[(warp * 2 + 1) * kCout + 8 * jb + cq + e] = s2[2 * jb + e];
+          }
       }
-      asm volatile("bar.sync 1, 128;\n" ::: "memory");
+      ptx::named_bar_sync(1, 32 * kConsumerWarps);
+      const int m = threadIdx.x;
       if (m < 2 * kCout) {
         const int which = m / kCout, ci = m - which * kCout;
         float a = 0.f;
 #pragma unroll
-        for (int w4 = 0; w4 < 4; ++w4) a += red[(w4 * 2 + which) * kCout + ci];
+        for (int w = 0; w < kConsumerWarps; ++w) a += red[(w * 2 + which) * kCout + ci];
         P.stats[(size_t)blockIdx.x * 2 * kCout + which * kCout + ci] = a;
       }
     }
-  }
-  ptx::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tcgen05_fence_after();
-    ptx::tmem_dealloc<kTmemCols>(tmem_base);
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // weight gradient: dW[co][kh][kw][ci] += sum_{n,y,x} dY[n,y,x,co] * X[n, y+kh-pad, x+kw-pad, ci]
 // One input row X[i] meets the KH gradient rows dY[i-KH+1 .. i] that use it: those rows sit in CONSECUTIVE ring slots
-// (the first KH-1 slots are mirrored behind the ring, so a window never wraps), which makes (row, Cout) one long N
-// dimension of a single MMA:  D[m = (kw shift, ci)][n = (dY row, co)] += X_row^T . dY_window,  K = 16 pixels.
-// TMEM block b of plane p (Cout columns at (p*KH + b)*Cout) holds kh = KH-1-b.  At the first/last rows of a chunk the
-// window is clipped to the chunk's own rows (narrower N, shifted block), so every (row, kh) pair is counted once.
-template <int KS, int CIN>
-__global__ void __launch_bounds__(192, 4)
+// (the first KH-1 slots are mirrored behind the ring, so a window never wraps).  Per input row and plane p:
+//   D_b[m = (kw shift, ci)][n = co] += X_row^T . dY_row(j),  K = 16 pixels,  for every dY row j of the window,
+// where accumulator b = KH-1-kh holds kh = i - j.  At the first/last rows of a chunk the window is clipped to the
+// chunk's own rows, so every (row, kh) pair is counted once.  Consumer warpgroup p owns input-channel plane p
+// (M = 8 shifts x 8 channels = 64; KW <= 7) and keeps its KH accumulators in registers for the CTA's lifetime.
+template <int KS, int CIN, int CO>
+__global__ void __launch_bounds__(CIN / 8 * 128 + 32, 1)
 conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_dy,
-                       const HaloParams P, const uint32_t tmem_cols_pow2) {
-  const int KH = KS > 0 ? KS : P.KH;
-  const int NP = CIN > 0 ? (CIN >> 3) : P.P;
+                       const HaloParams P) {
+  constexpr int KH = KS;
+  constexpr int NP = CIN >> 3;
+  constexpr int kWarps = 4 * NP;                            // consumer warps; warp kWarps = TMA producer
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
   constexpr int plane_bytes = 144 * 16;                     // P.BW == 144 always for the weight gradient
-  const int slot_bytes = NP * plane_bytes;
+  constexpr int slot_bytes = NP * plane_bytes;
   constexpr int dy_plane_bytes = 128 * 16;
-  const int dy_slot_bytes = P.PO * dy_plane_bytes;
+  constexpr int dy_slot_bytes = (CO / 8) * dy_plane_bytes;
   uint8_t* ring = smem;
   uint8_t* dyring = ring + (size_t)P.R * slot_bytes;                        // RD slots + KH-1 mirror slots
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(dyring + (size_t)(P.RD + KH - 1) * dy_slot_bytes);
   uint64_t* empty_bar = full_bar + P.R;
   uint64_t* dfull_bar = empty_bar + P.R;
   uint64_t* dempty_bar = dfull_bar + P.RD;
-  uint64_t* done_bar = dempty_bar + P.RD;
-  uint64_t* zero_bar = done_bar + 1;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(zero_bar + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) { ptx::prefetch_tensormap(&tmap_x); ptx::prefetch_tensormap(&tmap_dy); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < P.R; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < P.RD; ++s) { ptx::mbar_init(&dfull_bar[s], 1); ptx::mbar_init(&dempty_bar[s], 1); }
-    ptx::mbar_init(done_bar, 1);
-    ptx::mbar_init(zero_bar, 4);
+  if (warp == kWarps && lane == 0) {
+    ptx::prefetch_tensormap(&tmap_x); ptx::prefetch_tensormap(&tmap_dy);
+    for (int s = 0; s < P.R; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kWarps); }
+    for (int s = 0; s < P.RD; ++s) { ptx::mbar_init(&dfull_bar[s], 1); ptx::mbar_init(&dempty_bar[s], kWarps); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) {
-    if (tmem_cols_pow2 == 512) ptx::tmem_alloc<512>(tmem_ptr);
-    else if (tmem_cols_pow2 == 256) ptx::tmem_alloc<256>(tmem_ptr);
-    else ptx::tmem_alloc<128>(tmem_ptr);
-  }
-  ptx::tcgen05_fence_before();
   __syncthreads();
-  ptx::tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const int ncols = NP * KH * P.Cout;                        // multiple of 16
 
-  if (warp == 0) {
+  if (warp == kWarps) {
     if (ptx::elect_one()) {
       uint32_t slot = 0, par = 0, ds = 0, dpar = 0;
       for (int c = blockIdx.x; c < P.total_chunks; c += gridDim.x) {
@@ -348,7 +288,7 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_
             const bool mirror = ds < (uint32_t)(KH - 1);
             ptx::mbar_expect_tx(&dfull_bar[ds], (uint32_t)dy_slot_bytes * (mirror ? 2u : 1u));
             uint8_t* dd = dyring + (size_t)ds * dy_slot_bytes;
-            for (int p = 0; p < P.PO; ++p) {
+            for (int p = 0; p < CO / 8; ++p) {
               ptx::tma_load_4d(dd + p * dy_plane_bytes, &tmap_dy, &dfull_bar[ds], p * 8, x0, y0 + i, n);
               if (mirror)
                 ptx::tma_load_4d(dd + (size_t)P.RD * dy_slot_bytes + p * dy_plane_bytes, &tmap_dy, &dfull_bar[ds], p * 8, x0,
@@ -366,96 +306,81 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_
         }
       }
     }
-  } else if (warp == 1) {
-    if (ptx::elect_one()) {
-      const uint32_t idesc0 = ptx::make_idesc_bf16(128, 0, 1, 1);
-      const uint32_t R = (uint32_t)P.R, RD = (uint32_t)P.RD;
-      const uint32_t slot_u = (uint32_t)slot_bytes >> 4, dy_slot_u = (uint32_t)dy_slot_bytes >> 4;
-      // A: MN-major, MN chunk (pixel shift) stride 16 B ("SBO"), K group (8 px) stride 128 B ("LBO")
-      const uint32_t a_lo0 = (ptx::smem_u32(ring) >> 4) | (8u << 16);
-      // B: MN-major, MN chunk (8 output channels; planes of a row, then the next row's) stride = dY plane
-      const uint32_t b_lo0 = (ptx::smem_u32(dyring) >> 4) | (8u << 16);
-      constexpr uint32_t a_hi = halo_desc_hi(16), b_hi = halo_desc_hi(dy_plane_bytes);
-      uint32_t xslot = 0, xpar = 0;            // input-row FIFO
-      uint32_t dwait = 0, dwpar = 0;           // next dY slot to wait for
-      uint32_t dlo = 0;                        // ring slot of the oldest dY row still in use
-      ptx::mbar_wait(zero_bar, 0);             // accumulators were zeroed by the epilogue warps
-      ptx::tcgen05_fence_after();
-      for (int c = blockIdx.x; c < P.total_chunks; c += gridDim.x) {
-        const int cy = c % P.chunks_per_col;
-        const int y0 = cy * P.rows_per_chunk;
-        const int rows = min(P.rows_per_chunk, P.H - y0);
-        for (int i = 0; i < rows + KH - 1; ++i) {
-          if (i < rows) {
-            ptx::mbar_wait(&dfull_bar[dwait], dwpar);
-            if (++dwait == RD) { dwait = 0; dwpar ^= 1u; }
-          }
-          ptx::mbar_wait(&full_bar[xslot], xpar);
-          ptx::tcgen05_fence_after();
-          const int jlo = max(0, i - KH + 1), jhi = min(rows - 1, i);
-          const int nvalid = jhi - jlo + 1;
-          const int blo = KH - 1 - i + jlo;                  // TMEM block of dY row jlo (kh = i - jlo)
-          const uint32_t idesc = idesc0 | ((uint32_t)(nvalid * P.Cout) >> 3) << 17;
-          const uint32_t dy_lo = b_lo0 + dlo * dy_slot_u;    // dlo is the slot of row jlo (rows below jlo are released)
-          const uint32_t row_lo = a_lo0 + xslot * slot_u;
+  } else {
+    const int p = warp >> 2;                 // input-channel plane of this warpgroup
+    const uint32_t R = (uint32_t)P.R, RD = (uint32_t)P.RD;
+    constexpr uint32_t slot_u = (uint32_t)slot_bytes >> 4, dy_slot_u = (uint32_t)dy_slot_bytes >> 4;
+    // A: MN-major, MN chunk (pixel shift) stride 16 B ("SBO"), K group (8 px) stride 128 B ("LBO")
+    const uint32_t a_lo0 = ((ptx::smem_u32(ring) >> 4) + (uint32_t)(p * (plane_bytes >> 4))) | (8u << 16);
+    // B: MN-major, MN chunk (8 output channels) stride = dY plane
+    const uint32_t b_lo0 = (ptx::smem_u32(dyring) >> 4) | (8u << 16);
+    constexpr uint32_t a_hi = halo_desc_hi(16), b_hi = halo_desc_hi(dy_plane_bytes);
+    float acc[KH][CO / 2];
 #pragma unroll
-          for (int p = 0; p < NP; ++p) {
-            const uint32_t tacc = tmem_base + (uint32_t)((p * KH + blo) * P.Cout);
+    for (int b = 0; b < KH; ++b)
 #pragma unroll
-            for (int t = 0; t < 8; ++t)
-              ptx::umma_bf16(tacc, halo_desc(row_lo + (uint32_t)(p * (plane_bytes >> 4) + t * 16), a_hi),
-                             halo_desc(dy_lo + (uint32_t)(t * 16), b_hi), idesc, 1u);
-          }
-          ptx::umma_commit(&empty_bar[xslot]);
-          if (++xslot == R) { xslot = 0; xpar ^= 1u; }
-          if (i >= KH - 1) {                                 // dY row i-KH+1 has met its last input row
-            ptx::umma_commit(&dempty_bar[dlo]);
-            if (++dlo == RD) dlo = 0;
-          }
+      for (int i = 0; i < CO / 2; ++i) acc[b][i] = 0.f;
+    uint32_t xslot = 0, xpar = 0;            // input-row FIFO
+    uint32_t dwait = 0, dwpar = 0;           // next dY slot to wait for
+    uint32_t dlo = 0;                        // ring slot of the oldest dY row still in use
+    for (int c = blockIdx.x; c < P.total_chunks; c += gridDim.x) {
+      const int cy = c % P.chunks_per_col;
+      const int y0 = cy * P.rows_per_chunk;
+      const int rows = min(P.rows_per_chunk, P.H - y0);
+      for (int i = 0; i < rows + KH - 1; ++i) {
+        if (i < rows) {
+          ptx::mbar_wait(&dfull_bar[dwait], dwpar);
+          if (++dwait == RD) { dwait = 0; dwpar ^= 1u; }
+        }
+        ptx::mbar_wait(&full_bar[xslot], xpar);
+        const int jlo = max(0, i - KH + 1), jhi = min(rows - 1, i);
+        const int nvalid = jhi - jlo + 1;
+        const int blo = KH - 1 - i + jlo;                  // accumulator of dY row jlo (kh = i - jlo)
+        const uint32_t dy_lo = b_lo0 + dlo * dy_slot_u;    // dlo is the slot of row jlo (rows below jlo are released)
+        const uint32_t row_lo = a_lo0 + xslot * slot_u;
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int b = 0; b < KH; ++b) {
+          const int t = b - blo;                           // window row of accumulator b
+          if (t < 0 || t >= nvalid) continue;
+#pragma unroll
+          for (int k = 0; k < 8; ++k)
+            ptx::wgmma_bf16<CO, 1, 1>(acc[b], halo_desc(row_lo + (uint32_t)(k * 16), a_hi),
+                                       halo_desc(dy_lo + (uint32_t)t * dy_slot_u + (uint32_t)(k * 16), b_hi), 1u);
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+#pragma unroll
+        for (int b = 0; b < KH; ++b) ptx::fence_regs(acc[b]);
+        __syncwarp();
+        if (lane == 0) ptx::mbar_arrive(&empty_bar[xslot]);
+        if (++xslot == R) { xslot = 0; xpar ^= 1u; }
+        if (i >= KH - 1) {                                 // dY row i-KH+1 has met its last input row
+          if (lane == 0) ptx::mbar_arrive(&dempty_bar[dlo]);
+          if (++dlo == RD) dlo = 0;
         }
       }
-      ptx::umma_commit(done_bar);
     }
-  } else {
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int kw = m >> 3, cil = m & 7;
-    for (int c0 = 0; c0 < ncols; c0 += 16) ptx::tmem_st_32x32b_x16_fill(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, 0u);
-    ptx::tmem_st_wait();
-    ptx::tcgen05_fence_before();
-    __syncwarp();
-    if (lane == 0) ptx::mbar_arrive(zero_bar);
-    ptx::mbar_wait(done_bar, 0);
-    ptx::tcgen05_fence_after();
-    if (q * 4 < P.KW) {                      // warps whose 4 pixel shifts include a real tap
-      for (int p = 0; p < NP; ++p)
-        for (int b = 0; b < KH; ++b) {
-          const int kh = KH - 1 - b;
-          const int ci = p * 8 + cil;
-          for (int c0 = 0; c0 < P.Cout; c0 += 16) {
-            uint32_t v[16];
-            ptx::tmem_ld_32x32b_x16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)((p * KH + b) * P.Cout + c0), v);
-            ptx::tmem_ld_wait();
-            if (kw < P.KW) {
 #pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const int co = c0 + i;
-                const size_t off = P.oihw ? (((size_t)co * P.Cin + ci) * P.KH + kh) * P.KW + kw
-                                          : (((size_t)co * P.KH + kh) * P.KW + kw) * P.Cin + ci;
-                atomicAdd(P.dw + off, __uint_as_float(v[i]));
-              }
-            }
+    for (int h = 0; h < 2; ++h) {
+      const int m = (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      const int kw = m >> 3, ci = p * 8 + (m & 7);
+      if (kw >= P.KW) continue;
+#pragma unroll
+      for (int b = 0; b < KH; ++b) {
+        const int kh = KH - 1 - b;
+#pragma unroll
+        for (int jb = 0; jb < CO / 8; ++jb)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int co = 8 * jb + 2 * (lane & 3) + e;
+            const size_t off = P.oihw ? (((size_t)co * P.Cin + ci) * P.KH + kh) * P.KW + kw
+                                      : (((size_t)co * P.KH + kh) * P.KW + kw) * P.Cin + ci;
+            if (P.part) P.part[(size_t)blockIdx.x * P.welems + off] = acc[b][4 * jb + 2 * h + e];
+            else P.dw[off] += acc[b][4 * jb + 2 * h + e];
           }
-        }
+      }
     }
-  }
-  ptx::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tcgen05_fence_after();
-    if (tmem_cols_pow2 == 512) ptx::tmem_dealloc<512>(tmem_base);
-    else if (tmem_cols_pow2 == 256) ptx::tmem_dealloc<256>(tmem_base);
-    else ptx::tmem_dealloc<128>(tmem_base);
   }
 }
 
@@ -481,9 +406,8 @@ static bool halo_wgrad_eligible(const c3d_conv_desc* d) {
   if (!(d->Cin == 8 || d->Cin == 16 || d->Cin == 32)) return false;
   if (!(d->Cout == 16 || d->Cout == 32)) return false;
   if ((d->x_pix_stride != 0 && d->x_pix_stride != d->Cin) || (d->y_pix_stride != 0 && d->y_pix_stride != d->Cout)) return false;
-  if ((d->W < 128 && d->Cin != 8) || d->KH > 7) return false;
-  if (d->KH * (d->Cin / 8) * d->Cout > 512) return false;
-  return true;
+  if (d->W < 128 && d->Cin != 8) return false;
+  return (d->KH == 7 && d->Cin == 8) || (d->KH == 3 && d->Cin >= 16);     // the compiled instances
 }
 // ring depth: the TMA rows are only 2-4 KB, so hiding ~1.5 us of L2/HBM latency at ~40 B/ns per SM needs tens of rows in
 // flight; C3D_HALO_PREFETCH overrides the number of rows beyond the filter window
@@ -528,7 +452,7 @@ static int32_t launch_halo_fwd_inst(const CUtensorMap& mx, const HaloParams& P, 
     if (e != cudaSuccess) return set_error(C3D_ECUDA, "halo smem attr: %s", cudaGetErrorString(e));
     cur = smem;
   }
-  kern<<<grid, 192, smem, st>>>(mx, P);
+  kern<<<grid, kGemmThreads, smem, st>>>(mx, P);
   return check_launch("conv_halo_fwd_kernel");
 }
 
@@ -558,8 +482,8 @@ static int32_t launch_halo_fwd(const c3d_conv_desc* d, const void* x, const void
   CUresult r = halo_tensormap(enc, &mx, x, d->Cin, d->W, d->H, d->N, P.BW);
   if (r != CUDA_SUCCESS) return set_error(C3D_ECUDA, "encode halo x tensormap failed: %d", (int)r);
   const int wimg = (P.ksteps * d->Cout * 32 + 127) & ~127;
-  const size_t smem = 128 + (size_t)wimg + (size_t)P.R * P.P * P.BW * 16 + (size_t)(2 * P.R + 8) * 8 + 16 +
-                      4 * 2 * d->Cout * sizeof(float) + 64;
+  const size_t smem = 128 + (size_t)wimg + (size_t)P.R * P.P * P.BW * 16 + (size_t)(2 * P.R) * 8 +
+                      kConsumerWarps * 2 * d->Cout * sizeof(float) + 64;
   if (smem > 200 * 1024) return set_error(C3D_EINVAL, "halo conv: smem %zu too large", smem);
 #define C3D_HALO_F(ch, ks, cin) \
   if (d->Cout == ch * 16 && d->KH == ks && d->Cin == cin) return launch_halo_fwd_inst<ch, ks, cin>(mx, P, grid, smem, st);
@@ -574,18 +498,22 @@ static int32_t launch_halo_fwd(const c3d_conv_desc* d, const void* x, const void
   return launch_halo_fwd_inst<2, 0, 0>(mx, P, grid, smem, st);
 }
 
-template <int KS, int CIN>
+template <int KS, int CIN, int CO>
 static int32_t launch_halo_wgrad_inst(const CUtensorMap& mx, const CUtensorMap& mdy, const HaloParams& P, int grid, size_t smem,
-                                      uint32_t tcols, cudaStream_t st) {
-  auto kern = conv_halo_wgrad_kernel<KS, CIN>;
+                                      cudaStream_t st) {
+  auto kern = conv_halo_wgrad_kernel<KS, CIN, CO>;
   static size_t cur = 0;
   if (smem > cur) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return set_error(C3D_ECUDA, "halo wgrad smem attr: %s", cudaGetErrorString(e));
     cur = smem;
   }
-  kern<<<grid, 192, smem, st>>>(mx, mdy, P, tcols);
-  return check_launch("conv_halo_wgrad_kernel");
+  return with_ordered_partials(grid, P.welems, P.dw, st, [&](float* part) -> int32_t {
+    HaloParams Q = P;
+    Q.part = part;
+    kern<<<grid, CIN / 8 * 128 + 32, smem, st>>>(mx, mdy, Q);
+    return check_launch("conv_halo_wgrad_kernel");
+  });
 }
 
 static int32_t launch_halo_wgrad(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int oihw,
@@ -594,20 +522,18 @@ static int32_t launch_halo_wgrad(const c3d_conv_desc* d, const void* x, const vo
   if (!enc) return set_error(C3D_ECUDA, "cuTensorMapEncodeTiled unavailable");
   HaloParams P;
   memset(&P, 0, sizeof(P));
-  const int cols = d->KH * (d->Cin / 8) * d->Cout;
-  const uint32_t tcols = cols <= 128 ? 128u : (cols <= 256 ? 256u : 512u);
   P.N = d->N; P.H = d->H; P.W = d->W; P.Cin = d->Cin; P.Cout = d->Cout; P.KH = d->KH; P.KW = d->KW; P.pad = d->pad;
   P.P = d->Cin / 8; P.PO = d->Cout / 8;
   P.BW = 144;
   P.R = halo_ring_rows(0, P.P * P.BW * 16, 16 * 1024);             // input rows are a plain FIFO here
   P.RD = halo_ring_rows(d->KH, P.PO * 128 * 16, 0);                // window of KH rows + 2 in flight
   P.dw = dw; P.oihw = oihw;
+  P.welems = (long long)d->Cout * d->KH * d->KW * d->Cin;
   const size_t smem = 128 + (size_t)P.R * P.P * P.BW * 16 + (size_t)(P.RD + d->KH - 1) * P.PO * 128 * 16 +
-                      (size_t)(2 * P.R + 2 * P.RD + 2) * 8 + 16 + 64;
+                      (size_t)(2 * P.R + 2 * P.RD) * 8 + 64;
   if (smem > 200 * 1024) return set_error(C3D_EINVAL, "halo wgrad: smem %zu too large", smem);
-  int ctas = (int)(512u / tcols);                                  // co-resident CTAs: TMEM blocks, shared memory
-  const int by_smem = (int)((227 * 1024) / (smem + 1024));
-  if (ctas > by_smem) ctas = by_smem;
+  int ctas = (int)((227 * 1024) / (smem + 1024));                  // co-resident CTAs by shared memory
+  if (ctas > 4) ctas = 4;
   if (ctas < 1) ctas = 1;
   int grid;
   halo_chunking(d, &P, ctas, &grid);
@@ -616,10 +542,16 @@ static int32_t launch_halo_wgrad(const c3d_conv_desc* d, const void* x, const vo
   if (r != CUDA_SUCCESS) return set_error(C3D_ECUDA, "encode halo x tensormap failed: %d", (int)r);
   r = halo_tensormap(enc, &mdy, dy, d->Cout, d->W, d->H, d->N, 128);
   if (r != CUDA_SUCCESS) return set_error(C3D_ECUDA, "encode halo dy tensormap failed: %d", (int)r);
-  if (d->KH == 7 && d->Cin == 8) return launch_halo_wgrad_inst<7, 8>(mx, mdy, P, grid, smem, tcols, st);
-  if (d->KH == 3 && d->Cin == 16) return launch_halo_wgrad_inst<3, 16>(mx, mdy, P, grid, smem, tcols, st);
-  if (d->KH == 3 && d->Cin == 32) return launch_halo_wgrad_inst<3, 32>(mx, mdy, P, grid, smem, tcols, st);
-  return launch_halo_wgrad_inst<0, 0>(mx, mdy, P, grid, smem, tcols, st);
+#define C3D_HALO_W(ks, cin, co) \
+  if (d->KH == ks && d->Cin == cin && d->Cout == co) return launch_halo_wgrad_inst<ks, cin, co>(mx, mdy, P, grid, smem, st);
+  C3D_HALO_W(7, 8, 16)
+  C3D_HALO_W(7, 8, 32)
+  C3D_HALO_W(3, 16, 16)
+  C3D_HALO_W(3, 16, 32)
+  C3D_HALO_W(3, 32, 16)
+  C3D_HALO_W(3, 32, 32)
+#undef C3D_HALO_W
+  return set_error(C3D_EINVAL, "halo wgrad: no kernel for %dx%d, Cin %d, Cout %d", d->KH, d->KW, d->Cin, d->Cout);
 }
 
 }  // namespace c3d

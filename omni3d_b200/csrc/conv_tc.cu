@@ -1,4 +1,4 @@
-// conv_tc.cu — NHWC bf16 implicit-GEMM convolution on the 5th-gen tensor cores (sm_100a).
+// conv_tc.cu — NHWC bf16 implicit-GEMM convolution on the Hopper tensor cores (sm_90a, wgmma).
 //
 // Replaces the cuDNN convolutions the reference reaches through nn.Conv2d in
 //   cubercnn/modeling/backbone/dla.py:43-51,159-161,211-214,241-243,287-297 (DLA34 bottom-up),
@@ -6,35 +6,29 @@
 //   detectron2 StandardRPNHead (configs/Base.yaml:49)
 // for forward and (with flipped/transposed weights) data-gradient passes.
 //
-// GEMM view: M = output pixels, N = Cout, K = KH*KW*Cin.  One CTA computes a 128-pixel x BLOCK_N
-// tile.  A (activations): for every filter tap one 4-D TMA box [1][TH][TW][BLOCK_K] at the tap's
-// shifted coordinates — TMA out-of-bounds zero fill *is* the convolution padding and the
-// element-stride field *is* the convolution stride — landing in shared memory as the canonical
-// K-major 128B/64B/32B-swizzled UMMA operand (TH*TW <= 128 rows).  B (weights, [Cout][KH*KW*Cin]
-// bf16): 2-D TMA box.  tcgen05.mma (cta_group::1, M=128) accumulates in TMEM; warp-specialised:
-// warp0 = TMA producer, warp1 = MMA issuer, warps 2-5 = epilogue (tcgen05.ld -> bias / addend /
-// ReLU / BatchNorm partial statistics -> bf16|fp32 NHWC stores).
+// GEMM view: M = output pixels, N = Cout, K = KH*KW*Cin.  One CTA computes 128-pixel x BLOCK_N tiles.
+// A (activations): for every filter tap one 4-D TMA box [1][TH][TW][BLOCK_K] at the tap's shifted coordinates —
+// TMA out-of-bounds zero fill *is* the convolution padding and the element-stride field *is* the convolution
+// stride — landing in shared memory as the canonical K-major 128B/64B/32B-swizzled wgmma operand (TH*TW <= 128
+// rows).  B (weights, [Cout][KH*KW*Cin] bf16): 2-D TMA box.  Warp-specialised and persistent: warp 8 = TMA producer
+// over an mbarrier ring of STAGES slots; warps 0-7 = two consumer warpgroups, each accumulating 64 of the 128 tile
+// rows in registers with wgmma (M = 64, N = BLOCK_N) and running the epilogue of its rows (bias / addend / ReLU /
+// BatchNorm partial statistics -> bf16|fp32 NHWC stores) while the producer already streams the next tile.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include <string.h>
 #include "c3d_common.cuh"
-#include "ptx_sm100.cuh"
-
-// lab switches (tools/conv_lab.sh, tools/wgrad_lab.sh): compiled in only with -DC3D_LAB (libc3d_lab.so) — even a uniform
-// branch on a kernel parameter inside the pipeline loops cost the persistent kernel 14 % (profiles/r02_summary.md)
-#ifdef C3D_LAB
-#define C3D_DBG(P, bit) ((P).dbg & (bit))
-#else
-#define C3D_DBG(P, bit) (0)
-#endif
+#include "ptx_sm90.cuh"
 
 namespace c3d {
 
 using bf16 = __nv_bfloat16;
 
+constexpr int kConsumerWarps = 8;                       // two consumer warpgroups
+constexpr int kGemmThreads = 32 * kConsumerWarps + 32;  // + one TMA producer warp (warp 8)
+
 struct ConvKParams {
-  int dbg;                     // lab switches (C3D_CONV_DBG): 1 no MMA, 2 no TMA, 4 no B, 8 no A, 16 no epilogue
   int N, Ho, Wo, Cout;
   int KH, KW, stride, pad;
   int TH, TW, tiles_h, tiles_w;
@@ -43,7 +37,7 @@ struct ConvKParams {
   const float* bias;         // [Cout] or null
   int relu;
   int out_fp32;
-  int add_mode;              // 0 none, 1 same-size, 2 nearest-up2 (addend (N,Ho/2,Wo/2,add_pix_stride))
+  int add_mode;              // 0 none, 1 same-size, 2 nearest-up2 (addend (N,Ho/2,Wo/2,add_pix_stride)), 3 in place
   const bf16* addend;
   long long add_pix_stride;
   void* out;
@@ -58,259 +52,119 @@ template <int BLOCK_N, int BLOCK_K, int STAGES>
 struct ConvSmem {
   static constexpr int kABytes = 128 * BLOCK_K * 2;
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;       // both multiples of 1024 for BLOCK_N>=32|BK=64
+  static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kTileBytes = ((kStageBytes + 1023) / 1024) * 1024;
   static constexpr int kBarOffset = STAGES * kTileBytes;
-  static constexpr int kRedOffset = kBarOffset + 256;                      // BatchNorm partial sums [4 warps][2][256] fp32
-  static constexpr int kStgOffset = kRedOffset + 4 * 2 * 256 * 4;          // epilogue staging (BatchNorm transposes)
-  static constexpr int kTotal = kStgOffset + 4 * 16 * 33 * 4 + 1024 /*align slack*/;   // staging: 4 warps x 16 x 33 floats
+  static constexpr int kRedOffset = kBarOffset + 256;                      // BatchNorm partial sums [8 warps][2][BLOCK_N]
+  static constexpr int kTotal = kRedOffset + kConsumerWarps * 2 * BLOCK_N * 4 + 1024 /*align slack*/;
 };
 
-// ------------------------------------------------------------------------------------------------
-// Epilogue of one 128-pixel x BLOCK_N accumulator tile, run by the 4 epilogue warps (warp q owns TMEM lanes 32q..32q+31 =
-// tile rows = output pixels): tcgen05.ld 16 columns at a time -> BatchNorm partial sums -> bias / addend / ReLU ->
-// bf16|fp32 NHWC store (a thread owns one pixel = one row of the output and writes its 16 channels as 2 x 16 bytes).
-// Shared by the one-tile-per-CTA and the persistent kernel.
+// Epilogue of the 64 rows (output pixels) of a 128 x BLOCK_N tile that consumer warpgroup `wg` accumulated.  A thread
+// holds two pixels (rows 16w + l/4 and +8) and, per 8-channel block j, the channel pair 8j + 2(l%4): every store is a
+// bf16x2 / float2 of one pixel; the four lanes of a quad cover 8 consecutive channels.
 template <int BLOCK_N>
-__device__ __forceinline__ void conv_epilogue_tile(const ConvKParams& P, const uint32_t tacc /*TMEM address incl. lane*/,
-                                                   const int q, const int lane, const int img, const int ho0, const int wo0,
-                                                   const int n0, const int tile_m, float* red, uint8_t* stg_all) {
-  const int r = q * 32 + lane;                 // tile row = TMEM lane
-  const int ty = r / P.TW, tx = r - ty * P.TW;
-  const int ho = ho0 + ty, wo = wo0 + tx;
-  const bool valid = (r < P.TH * P.TW) && (ho < P.Ho) && (wo < P.Wo);
-  const long long lpix = ((long long)img * P.Ho + ho) * P.Wo + wo;   // dense pixel index (addend / stats)
-  const long long pix = (long long)img * P.out_img_stride + (long long)ho * P.out_h_stride + (long long)wo * P.out_w_stride + P.out_off;
-  long long apix = 0;
-  if (P.add_mode == 1) apix = lpix;
-  else if (P.add_mode == 2) apix = ((long long)img * (P.Ho >> 1) + (ho >> 1)) * (P.Wo >> 1) + (wo >> 1);
-  constexpr int kChunks = (BLOCK_N + 15) / 16;
-  constexpr int kStatN = kChunks * 16;
-  // TMEM loads are software-pipelined: chunk ch+1 is in flight while chunk ch is reduced / converted / stored
-  uint32_t v[16];
-  ptx::tmem_ld_32x32b_x16(tacc, v);
-#pragma unroll 1
-  for (int ch = 0; ch < kChunks; ++ch) {
-    ptx::tmem_ld_wait();
-    float f[16];
+__device__ __forceinline__ void conv_epilogue_tile(const ConvKParams& P, const float (&acc)[BLOCK_N / 2], const int warp,
+                                                   const int lane, const int img, const int ho0, const int wo0,
+                                                   const int n0, const int tile_m, float* red) {
+  bool valid[2];
+  long long pix[2], apix[2];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[i]);
-    if (ch + 1 < kChunks) ptx::tmem_ld_32x32b_x16(tacc + (uint32_t)((ch + 1) * 16), v);
-    const int c0 = n0 + ch * 16;
-    const long long coff = c0 + ((P.split_c && c0 >= P.split_c) ? P.split_off : 0);   // channel offset inside the pixel
+  for (int h = 0; h < 2; ++h) {
+    const int r = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    const int ty = r / P.TW, tx = r - ty * P.TW;
+    const int ho = ho0 + ty, wo = wo0 + tx;
+    valid[h] = (r < P.TH * P.TW) && (ho < P.Ho) && (wo < P.Wo);
+    pix[h] = (long long)img * P.out_img_stride + (long long)ho * P.out_h_stride + (long long)wo * P.out_w_stride + P.out_off;
+    apix[h] = 0;
+    if (P.add_mode == 1) apix[h] = ((long long)img * P.Ho + ho) * P.Wo + wo;
+    else if (P.add_mode == 2) apix[h] = ((long long)img * (P.Ho >> 1) + (ho >> 1)) * (P.Wo >> 1) + (wo >> 1);
+  }
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int c = n0 + 8 * j + cq;                                   // channel pair (c, c + 1)
     if (P.stats) {
-      // per-channel sum / sum-of-squares over the valid rows of this tile (raw fp32 accumulators).  Each warp transposes its
-      // 32 rows x 16 channels through a private 16 x 33-word shared-memory tile (row r writes column r: conflict-free; lane
-      // (c = l & 15, h = l >> 4) then sums rows 16h..16h+15 of channel c: banks (c + 16h + j) mod 32 are all distinct) and
-      // parks its 16 column sums in red[warp][.][channel]; the four warps are combined ONCE per tile after the chunk loop
-      // (two named barriers per tile instead of two per 16 channels).  Fixed summation order => deterministic.
-      float* tr = reinterpret_cast<float*>(stg_all) + q * (16 * 33);
+      // per-channel sum / sum of squares over the valid rows (raw fp32 accumulators): the two rows of a thread, then
+      // the 8 row groups of the warp (lanes with equal l%4); fixed order => deterministic
+      const float a0 = valid[0] ? acc[4 * j] : 0.f, a1 = valid[0] ? acc[4 * j + 1] : 0.f;
+      const float b0 = valid[1] ? acc[4 * j + 2] : 0.f, b1 = valid[1] ? acc[4 * j + 3] : 0.f;
+      float s0 = a0 + b0, s1 = a1 + b1, q0 = a0 * a0 + b0 * b0, q1 = a1 * a1 + b1 * b1;
 #pragma unroll
-      for (int i = 0; i < 16; ++i) tr[i * 33 + lane] = valid ? f[i] : 0.f;
-      __syncwarp();
-      const int c = lane & 15, h = lane >> 4;
-      float sa = 0.f, sb = 0.f;
-#pragma unroll
-      for (int j = 0; j < 16; ++j) { const float x = tr[c * 33 + h * 16 + j]; sa += x; sb += x * x; }
-      sa += __shfl_xor_sync(0xffffffffu, sa, 16);
-      sb += __shfl_xor_sync(0xffffffffu, sb, 16);
-      __syncwarp();
-      if (lane < 16) { red[(q * 2 + 0) * kStatN + ch * 16 + lane] = sa; red[(q * 2 + 1) * kStatN + ch * 16 + lane] = sb; }
-    }
-    const bool live = valid && c0 < P.Cout;
-    if (live) {
-      if (P.bias) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) f[i] += __ldg(P.bias + c0 + i);
+      for (int o = 4; o < 32; o <<= 1) {
+        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+        q1 += __shfl_xor_sync(0xffffffffu, q1, o);
       }
+      if (lane < 4) {
+        float* rs = red + (warp * 2) * BLOCK_N + 8 * j + cq;
+        rs[0] = s0; rs[1] = s1; rs[BLOCK_N] = q0; rs[BLOCK_N + 1] = q1;
+      }
+    }
+    if (c >= P.Cout) continue;
+    const long long coff = c + ((P.split_c && c >= P.split_c) ? P.split_off : 0);   // channel offset inside the pixel
+    float2 bv = make_float2(0.f, 0.f);
+    if (P.bias) bv = make_float2(__ldg(P.bias + c), __ldg(P.bias + c + 1));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!valid[h]) continue;
+      float v0 = acc[4 * j + 2 * h] + bv.x, v1 = acc[4 * j + 2 * h + 1] + bv.y;
       if (P.add_mode) {
-        const bf16* abase = P.add_mode == 3 ? reinterpret_cast<const bf16*>(P.out) + pix * P.out_pix_stride + (coff - c0)
-                                            : P.addend + apix * P.add_pix_stride;
-        const uint4* ap = reinterpret_cast<const uint4*>(abase + c0);
-        uint4 a0 = __ldg(ap), a1 = __ldg(ap + 1);
-        const bf16* h0 = reinterpret_cast<const bf16*>(&a0);
-        const bf16* h1 = reinterpret_cast<const bf16*>(&a1);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { f[i] += __bfloat162float(h0[i]); f[8 + i] += __bfloat162float(h1[i]); }
+        const bf16* ap = P.add_mode == 3 ? reinterpret_cast<const bf16*>(P.out) + pix[h] * P.out_pix_stride + coff
+                                         : P.addend + apix[h] * P.add_pix_stride + c;
+        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ap));
+        v0 += a.x; v1 += a.y;
       }
-      if (P.relu) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) f[i] = fmaxf(f[i], 0.f);
-      }
-    }
-    if (P.out_fp32) {
-      if (live) {
-        float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(P.out) + pix * P.out_pix_stride + coff);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) op[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-      }
-      continue;
-    }
-    uint32_t pk[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      __nv_bfloat162 h = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-      pk[i] = *reinterpret_cast<uint32_t*>(&h);
-    }
-    // direct 2 x 16-byte row stores (measured, profiles/r02: staging the tile through shared memory to write complete
-    // 128-byte row segments is SLOWER — 1x1 64->256 @160: 0.38 -> 0.72 ms; the write path already merges the two half-sector
-    // stores and the extra shared-memory round trip only lengthens a latency-bound epilogue)
-    if (live) {
-      uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(P.out) + pix * P.out_pix_stride + coff);
-      op[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      op[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+      if (P.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      if (P.out_fp32)
+        *reinterpret_cast<float2*>(reinterpret_cast<float*>(P.out) + pix[h] * P.out_pix_stride + coff) = make_float2(v0, v1);
+      else
+        *reinterpret_cast<__nv_bfloat162*>(reinterpret_cast<bf16*>(P.out) + pix[h] * P.out_pix_stride + coff) =
+            __floats2bfloat162_rn(v0, v1);
     }
   }
   if (P.stats) {
-    asm volatile("bar.sync 1, 128;\n" ::: "memory");
+    ptx::named_bar_sync(1, 32 * kConsumerWarps);
     float* dst = P.stats + (size_t)tile_m * 2 * P.Cout;
-    for (int i = q * 32 + lane; i < 2 * kStatN; i += 128) {
-      const int which = i / kStatN, cc = i - which * kStatN;
-      if (n0 + cc < P.Cout)
-        dst[which * P.Cout + n0 + cc] = ((red[(0 * 2 + which) * kStatN + cc] + red[(1 * 2 + which) * kStatN + cc]) +
-                                         red[(2 * 2 + which) * kStatN + cc]) + red[(3 * 2 + which) * kStatN + cc];
+    for (int i = threadIdx.x; i < 2 * BLOCK_N; i += 32 * kConsumerWarps) {
+      const int which = i / BLOCK_N, cc = i - which * BLOCK_N;
+      float a = 0.f;
+#pragma unroll
+      for (int w = 0; w < kConsumerWarps; ++w) a += red[(w * 2 + which) * BLOCK_N + cc];
+      if (n0 + cc < P.Cout) dst[which * P.Cout + n0 + cc] = a;
     }
-    asm volatile("bar.sync 1, 128;\n" ::: "memory");       // red / the transposes are reused by this CTA's next tile
+    ptx::named_bar_sync(1, 32 * kConsumerWarps);       // red is reused by this CTA's next tile
   }
 }
 
-
-template <int BLOCK_N, int BLOCK_K, int STAGES>
-__global__ void __launch_bounds__(192)
+// Persistent kernel: CTA b walks the (m-tile, n-tile) work items b, b + gridDim.x, ...  The stage ring runs across tile
+// boundaries, so the producer loads the next tile while the consumers are in the epilogue of the current one.
+template <int BLOCK_N, int BLOCK_K, int STAGES, int CPS>
+__global__ void __launch_bounds__(kGemmThreads, CPS)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-               const ConvKParams P) {
+               const ConvKParams P, const int tiles_m, const int n_tiles) {
   using S = ConvSmem<BLOCK_N, BLOCK_K, STAGES>;
   constexpr int kSwizzle = BLOCK_K * 2;                       // bytes per smem row = swizzle span
-  constexpr uint32_t kTmemCols = BLOCK_N < 32 ? 32 : BLOCK_N; // power of two >= 32
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-  float* red = reinterpret_cast<float*>(smem + S::kRedOffset);           // [4 warps][2][16]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  // tile coordinates
-  const int tile_m = blockIdx.x;
-  const int tw_i = tile_m % P.tiles_w;
-  const int th_i = (tile_m / P.tiles_w) % P.tiles_h;
-  const int img = tile_m / (P.tiles_w * P.tiles_h);
-  const int ho0 = th_i * P.TH, wo0 = tw_i * P.TW;
-  const int n0 = blockIdx.y * BLOCK_N;
-  const int num_kb = P.KH * P.KW * P.kc_blocks;
-
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tensormap(&tmap_x);
-    ptx::prefetch_tensormap(&tmap_w);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    ptx::mbar_init(tmem_full_bar, 1);
-    ptx::fence_barrier_init();
-  }
-  if (warp == 2) ptx::tmem_alloc<kTmemCols>(tmem_ptr);
-  ptx::tcgen05_fence_before();
-  __syncthreads();
-  ptx::tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ===== TMA producer =====
-    if (ptx::elect_one()) {
-      const uint32_t a_bytes = (uint32_t)(P.TH * P.TW * BLOCK_K * 2);
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int tap = kb / P.kc_blocks, kc = kb - tap * P.kc_blocks;
-        const int kh = tap / P.KW, kw = tap - kh * P.KW;
-        ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * S::kTileBytes;
-        uint8_t* sb = sa + S::kABytes;
-        ptx::mbar_expect_tx(&full_bar[stage], a_bytes + (uint32_t)S::kBBytes);
-        ptx::tma_load_4d(sa, &tmap_x, &full_bar[stage], kc * BLOCK_K, wo0 * P.stride + kw - P.pad,
-                         ho0 * P.stride + kh - P.pad, img);
-        ptx::tma_load_2d(sb, &tmap_w, &full_bar[stage], tap * P.Cin + kc * BLOCK_K, n0);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (ptx::elect_one()) {
-      constexpr uint32_t idesc = ptx::make_idesc_bf16(128, BLOCK_N < 16 ? 16 : BLOCK_N, 0, 0);
-      constexpr uint32_t lt = ptx::swizzle_layout_type(kSwizzle);
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        ptx::mbar_wait(&full_bar[stage], phase);
-        ptx::tcgen05_fence_after();
-        const uint32_t sa = ptx::smem_u32(smem + stage * S::kTileBytes);
-        const uint32_t sb = sa + S::kABytes;
-        const uint64_t da = ptx::make_smem_desc(sa, 16, 8 * kSwizzle, lt);
-        const uint64_t db = ptx::make_smem_desc(sb, 16, 8 * kSwizzle, lt);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) {
-          // advance 16 bf16 = 32 bytes along K inside the swizzle span: +2 in the (addr>>4) field
-          ptx::umma_bf16(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        ptx::umma_commit(&empty_bar[stage]);     // frees the smem slot when these MMAs retire
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      ptx::umma_commit(tmem_full_bar);           // accumulator complete
-    }
-  } else {
-    // ===== epilogue warps 2..5: TMEM lane quarter = warp % 4 =====
-    const int q = warp & 3;
-    ptx::mbar_wait(tmem_full_bar, 0);
-    ptx::tcgen05_fence_after();
-    conv_epilogue_tile<BLOCK_N>(P, tmem_base + ((uint32_t)(q * 32) << 16), q, lane, img, ho0, wo0, n0, tile_m, red,
-                                smem + S::kStgOffset);
-  }
-  ptx::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tcgen05_fence_after();
-    ptx::tmem_dealloc<kTmemCols>(tmem_base);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Persistent variant: one CTA per SM slot loops over (m-tile, n-tile) work items; the fp32 accumulator is
-// DOUBLE-BUFFERED in TMEM (2 x BLOCK_N columns) so the epilogue of tile i overlaps the TMA/MMA main loop of
-// tile i+1, and barrier init / TMEM allocation are paid once per CTA instead of once per 128-pixel tile.
-template <int BLOCK_N, int BLOCK_K, int STAGES>
-__global__ void __launch_bounds__(192)
-conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                          const ConvKParams P, const int tiles_m, const int n_tiles) {
-  using S = ConvSmem<BLOCK_N, BLOCK_K, STAGES>;
-  constexpr int kSwizzle = BLOCK_K * 2;
-  constexpr uint32_t kAccCols = BLOCK_N < 16 ? 16 : BLOCK_N;
-  constexpr uint32_t kTmemCols = (2 * kAccCols) < 32 ? 32 : (2 * kAccCols);
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;          // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;              // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty_bar + 2);
   float* red = reinterpret_cast<float*>(smem + S::kRedOffset);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = P.KH * P.KW * P.kc_blocks;
   const int total = tiles_m * n_tiles;
 
-  if (warp == 0 && lane == 0) { ptx::prefetch_tensormap(&tmap_x); ptx::prefetch_tensormap(&tmap_w); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { ptx::mbar_init(&tfull_bar[a], 1); ptx::mbar_init(&tempty_bar[a], 4); }
+  if (warp == kConsumerWarps && lane == 0) {
+    ptx::prefetch_tensormap(&tmap_x);
+    ptx::prefetch_tensormap(&tmap_w);
+    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kConsumerWarps); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) ptx::tmem_alloc<kTmemCols>(tmem_ptr);
-  ptx::tcgen05_fence_before();
   __syncthreads();
-  ptx::tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
+    // ===== TMA producer =====
     if (ptx::elect_one()) {
       const uint32_t a_bytes = (uint32_t)(P.TH * P.TW * BLOCK_K * 2);
       int stage = 0; uint32_t phase = 0;
@@ -319,312 +173,51 @@ conv_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gr
         const int tw_i = tile_m % P.tiles_w, th_i = (tile_m / P.tiles_w) % P.tiles_h;
         const int img = tile_m / (P.tiles_w * P.tiles_h);
         const int hi0 = th_i * P.TH * P.stride - P.pad, wi0 = tw_i * P.TW * P.stride - P.pad;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          const int tap = kb / P.kc_blocks, kc = kb - tap * P.kc_blocks;
-          const int kh = tap / P.KW, kw = tap - kh * P.KW;
-          ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * S::kTileBytes;
-          if C3D_DBG(P, 2) { ptx::mbar_arrive(&full_bar[stage]); if (++stage == STAGES) { stage = 0; phase ^= 1; } continue; }
-          ptx::mbar_expect_tx(&full_bar[stage], (C3D_DBG(P, 8) ? 0u : a_bytes) + (C3D_DBG(P, 4) ? 0u : (uint32_t)S::kBBytes));
-          if (!C3D_DBG(P, 8)) ptx::tma_load_4d(sa, &tmap_x, &full_bar[stage], kc * BLOCK_K, wi0 + kw, hi0 + kh, img);
-          if (!C3D_DBG(P, 4)) ptx::tma_load_2d(sa + S::kABytes, &tmap_w, &full_bar[stage], tap * P.Cin + kc * BLOCK_K, n0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (ptx::elect_one()) {
-      constexpr uint32_t idesc = ptx::make_idesc_bf16(128, kAccCols, 0, 0);
-      constexpr uint32_t lt = ptx::swizzle_layout_type(kSwizzle);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-        ptx::mbar_wait(&tempty_bar[acc], acc_phase ^ 1);      // epilogue drained this accumulator
-        ptx::tcgen05_fence_after();
-        const uint32_t tacc = tmem_base + (uint32_t)acc * kAccCols;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          if C3D_DBG(P, 1) { ptx::mbar_arrive(&empty_bar[stage]); if (++stage == STAGES) { stage = 0; phase ^= 1; } continue; }
-          ptx::tcgen05_fence_after();
-          const uint32_t sa = ptx::smem_u32(smem + stage * S::kTileBytes);
-          const uint64_t da = ptx::make_smem_desc(sa, 16, 8 * kSwizzle, lt);
-          const uint64_t db = ptx::make_smem_desc(sa + S::kABytes, 16, 8 * kSwizzle, lt);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k)
-            ptx::umma_bf16(tacc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-          ptx::umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::umma_commit(&tfull_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-      const int tile_m = tile / n_tiles, n0 = (tile - tile_m * n_tiles) * BLOCK_N;
-      const int tw_i = tile_m % P.tiles_w, th_i = (tile_m / P.tiles_w) % P.tiles_h;
-      const int img = tile_m / (P.tiles_w * P.tiles_h);
-      ptx::mbar_wait(&tfull_bar[acc], acc_phase);
-      ptx::tcgen05_fence_after();
-      if (!C3D_DBG(P, 16))
-      conv_epilogue_tile<BLOCK_N>(P, tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * kAccCols, q, lane, img,
-                                  th_i * P.TH, tw_i * P.TW, n0, tile_m, red, smem + S::kStgOffset);
-      // this warp is done reading the accumulator: hand it back to the MMA issuer
-      ptx::tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-  ptx::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tcgen05_fence_after();
-    ptx::tmem_dealloc<kTmemCols>(tmem_base);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// "Swapped" persistent kernel for layers with <= 128 output channels.  A tcgen05.mma with M = 128, K = 16 streams its A tile
-// (128 x 32 B) from shared memory in ~128 cycles whatever N is (measured with the pipeline lab, profiles/r02_summary.md: the
-// MMA-only loop costs ~520 cycles per 64-deep K block for N = 64, 128 and 256 alike), so D[pixels][Cout] with N = Cout = 128
-// (64) runs the tensor pipe at 50 % (25 %).  Here the roles are swapped: D[Cout (M = 128)][256 pixels (N)] — A = the weight
-// tile, B = a 256-pixel input tile — full rate for Cout = 128 and twice the old rate for Cout = 64 (rows 64..127 of A are
-// never loaded nor read back).  The accumulator is transposed (TMEM lane = output channel, column = pixel): an epilogue
-// thread owns ONE channel, so the BatchNorm partial sums need no cross-thread reduction, and for every pixel the 32 lanes of
-// a warp write 32 consecutive channels (64 B).
-struct ConvSwapSmem {
-  static constexpr int kStages = 4;
-  static constexpr int kWBytes = 128 * 64 * 2;        // weights  [128 co][64 k]
-  static constexpr int kXBytes = 256 * 64 * 2;        // pixels   [256 px][64 k]
-  static constexpr int kTileBytes = kWBytes + kXBytes;
-  static constexpr int kBarOffset = kStages * kTileBytes;
-  static constexpr int kStgOffset = kBarOffset + 256;        // epilogue transposes: 8 warps x [16 px][kStgPitch] fp32
-  static constexpr int kStgPitch = 36;                        // 32 channels + 4: 16-byte aligned rows, <= 2-way bank conflicts
-  static constexpr int kEpiWarps = 8;                         // two per TMEM lane quarter: pixel columns 0..127 / 128..255
-  static constexpr int kStatOffset = kStgOffset + kEpiWarps * 16 * kStgPitch * 4;   // [2][128] fp32: statistics of the upper half
-  static constexpr int kTotal = kStatOffset + 2 * 128 * 4 + 1024;
-  static constexpr int kThreads = 64 + 32 * kEpiWarps;
-};
-
-__global__ void __launch_bounds__(ConvSwapSmem::kThreads)
-conv_tc_swap_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                    const ConvKParams P, const int tiles_m) {
-  using S = ConvSwapSmem;
-  constexpr int STAGES = S::kStages;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;          // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;              // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_kb = P.KH * P.KW * P.kc_blocks;
-  const int wrows = P.Cout < 128 ? P.Cout : 128;
-
-  if (warp == 0 && lane == 0) { ptx::prefetch_tensormap(&tmap_x); ptx::prefetch_tensormap(&tmap_w); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { ptx::mbar_init(&tfull_bar[a], 1); ptx::mbar_init(&tempty_bar[a], ConvSwapSmem::kEpiWarps); }
-    ptx::fence_barrier_init();
-  }
-  if (warp == 2) ptx::tmem_alloc<512>(tmem_ptr);
-  ptx::tcgen05_fence_before();
-  __syncthreads();
-  ptx::tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (ptx::elect_one()) {
-      const uint32_t bytes = (uint32_t)(P.TH * P.TW * 64 * 2) + (uint32_t)(wrows * 64 * 2);
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < tiles_m; tile += gridDim.x) {
-        const int tw_i = tile % P.tiles_w, th_i = (tile / P.tiles_w) % P.tiles_h;
-        const int img = tile / (P.tiles_w * P.tiles_h);
-        const int hi0 = th_i * P.TH * P.stride - P.pad, wi0 = tw_i * P.TW * P.stride - P.pad;
         int tap = 0, kc = 0, kh = 0, kw = 0;
         for (int kb = 0; kb < num_kb; ++kb) {
           ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sw = smem + stage * S::kTileBytes;
-          ptx::mbar_expect_tx(&full_bar[stage], bytes);
-          ptx::tma_load_4d(sw + S::kWBytes, &tmap_x, &full_bar[stage], kc * 64, wi0 + kw, hi0 + kh, img);
-          ptx::tma_load_2d(sw, &tmap_w, &full_bar[stage], tap * P.Cin + kc * 64, 0);
+          uint8_t* sa = smem + stage * S::kTileBytes;
+          ptx::mbar_expect_tx(&full_bar[stage], a_bytes + (uint32_t)S::kBBytes);
+          ptx::tma_load_4d(sa, &tmap_x, &full_bar[stage], kc * BLOCK_K, wi0 + kw, hi0 + kh, img);
+          ptx::tma_load_2d(sa + S::kABytes, &tmap_w, &full_bar[stage], tap * P.Cin + kc * BLOCK_K, n0);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
           if (++kc == P.kc_blocks) { kc = 0; ++tap; if (++kw == P.KW) { kw = 0; ++kh; } }
         }
       }
     }
-  } else if (warp == 1) {
-    if (ptx::elect_one()) {
-      constexpr uint32_t idesc = ptx::make_idesc_bf16(128, 256, 0, 0);
-      constexpr uint32_t lt = ptx::swizzle_layout_type(128);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < tiles_m; tile += gridDim.x) {
-        ptx::mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        ptx::tcgen05_fence_after();
-        const uint32_t tacc = tmem_base + (uint32_t)acc * 256u;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          ptx::tcgen05_fence_after();
-          const uint32_t sw = ptx::smem_u32(smem + stage * S::kTileBytes);
-          const uint64_t da = ptx::make_smem_desc(sw, 16, 8 * 128, lt);
-          const uint64_t db = ptx::make_smem_desc(sw + S::kWBytes, 16, 8 * 128, lt);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            ptx::umma_bf16(tacc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-          ptx::umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::umma_commit(&tfull_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // 8 epilogue warps: warps (2 + q) and (6 + q') ... a warp may only read the TMEM lane quarter (warp & 3); the two warps of
-    // a quarter split the 256 pixel columns in halves, so every scheduler holds two epilogue warps to overlap the
-    // TMEM-load / shared-memory-transpose / store latencies of one with the other.
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;                  // 0: pixels 0..127, 1: pixels 128..255
-    const int co = q * 32 + lane;                      // TMEM lane = output channel
-    const bool cvalid = co < P.Cout;
-    const float bias = (P.bias && cvalid) ? __ldg(P.bias + co) : 0.f;
-    const int npix = P.TH * P.TW;
-    // store side of the transposes below: this thread writes pixel (lane >> 1) of a 16-pixel chunk, channels cs..cs+15
-    const int sp = lane >> 1, cs = q * 32 + (lane & 1) * 16;
-    const bool svalid = cs < P.Cout;
-    const long long csoff = cs + ((P.split_c && cs >= P.split_c) ? P.split_off : 0);      // channel offset inside the pixel
-    float* tr = reinterpret_cast<float*>(smem + S::kStgOffset) + (warp - 2) * (16 * S::kStgPitch);
-    float* sstat = reinterpret_cast<float*>(smem + S::kStatOffset);
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < tiles_m; tile += gridDim.x) {
-      const int tw_i = tile % P.tiles_w, th_i = (tile / P.tiles_w) % P.tiles_h;
-      const int img = tile / (P.tiles_w * P.tiles_h);
-      const int ho0 = th_i * P.TH, wo0 = tw_i * P.TW;
-      const bool full = (npix == 256) && (ho0 + P.TH <= P.Ho) && (wo0 + P.TW <= P.Wo);   // no pixel of the tile is masked
-      ptx::mbar_wait(&tfull_bar[acc], acc_phase);
-      ptx::tcgen05_fence_after();
-      const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * 256u + (uint32_t)half * 128u;
-      float ssum = 0.f, ssq = 0.f;
-      // (ty, tx) of the pixel this thread stores in the current chunk, advanced by 16 pixels per chunk
-      int sty = (half * 128 + sp) / P.TW, stx = (half * 128 + sp) - sty * P.TW;
-      uint32_t v[16];
-      ptx::tmem_ld_32x32b_x16(tacc, v);
-#pragma unroll 1
-      for (int ch = 0; ch < 8; ++ch) {
-        ptx::tmem_ld_wait();
-        float f[16];
+    // ===== consumer warpgroups: rows 64 * (warp / 4) .. +63 of every tile =====
+    constexpr uint32_t lt = ptx::swizzle_layout_type(kSwizzle);
+    const uint32_t a_row0 = (uint32_t)((warp >> 2) * 64 * kSwizzle);
+    float acc[BLOCK_N / 2];
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+      const int tile_m = tile / n_tiles, n0 = (tile - tile_m * n_tiles) * BLOCK_N;
+      const int tw_i = tile_m % P.tiles_w, th_i = (tile_m / P.tiles_w) % P.tiles_h;
+      const int img = tile_m / (P.tiles_w * P.tiles_h);
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        ptx::mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = ptx::smem_u32(smem + stage * S::kTileBytes);
+        const uint64_t da = ptx::make_smem_desc(sa + a_row0, 16, 8 * kSwizzle, lt);
+        const uint64_t db = ptx::make_smem_desc(sa + S::kABytes, 16, 8 * kSwizzle, lt);
+        ptx::wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[i]);
-        if (ch + 1 < 8) ptx::tmem_ld_32x32b_x16(tacc + (uint32_t)((ch + 1) * 16), v);
-        const int p0 = half * 128 + ch * 16;
-        if (p0 < npix) {                                // (warp-uniform) tile smaller than 256 pixels
-          if (P.stats) {                                // raw accumulators of the valid pixels; this thread owns channel co
-            if (full) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) { ssum += f[i]; ssq = fmaf(f[i], f[i], ssq); }
-            } else {
-              int ty = p0 / P.TW, tx = p0 - ty * P.TW;
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                if ((p0 + i < npix) && (ho0 + ty < P.Ho) && (wo0 + tx < P.Wo)) { ssum += f[i]; ssq = fmaf(f[i], f[i], ssq); }
-                if (++tx == P.TW) { tx = 0; ++ty; }
-              }
-            }
-          }
-          // transpose 32 channels x 16 pixels through shared memory so that a thread stores 16 consecutive channels of one
-          // pixel (2 x 16 B) instead of one 2-byte element per pixel
-#pragma unroll
-          for (int i = 0; i < 16; ++i) tr[i * S::kStgPitch + lane] = f[i] + bias;
-          __syncwarp();
-          const int ho = ho0 + sty, wo = wo0 + stx;
-          if (svalid && (p0 + sp) < npix && ho < P.Ho && wo < P.Wo) {
-            float g[16];
-            const float4* src = reinterpret_cast<const float4*>(tr + sp * S::kStgPitch + (lane & 1) * 16);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) { const float4 t4 = src[k]; g[4 * k] = t4.x; g[4 * k + 1] = t4.y; g[4 * k + 2] = t4.z; g[4 * k + 3] = t4.w; }
-            const long long pix = (long long)img * P.out_img_stride + (long long)ho * P.out_h_stride +
-                                  (long long)wo * P.out_w_stride + P.out_off;
-            if (P.add_mode) {
-              const bf16* abase;
-              if (P.add_mode == 3) abase = reinterpret_cast<const bf16*>(P.out) + pix * P.out_pix_stride + (csoff - cs);
-              else if (P.add_mode == 1) abase = P.addend + (((long long)img * P.Ho + ho) * P.Wo + wo) * P.add_pix_stride;
-              else abase = P.addend + (((long long)img * (P.Ho >> 1) + (ho >> 1)) * (P.Wo >> 1) + (wo >> 1)) * P.add_pix_stride;
-              const uint4* ap = reinterpret_cast<const uint4*>(abase + cs);
-              const uint4 a0 = __ldg(ap), a1 = __ldg(ap + 1);
-              const bf16* h0 = reinterpret_cast<const bf16*>(&a0);
-              const bf16* h1 = reinterpret_cast<const bf16*>(&a1);
-#pragma unroll
-              for (int k = 0; k < 8; ++k) { g[k] += __bfloat162float(h0[k]); g[8 + k] += __bfloat162float(h1[k]); }
-            }
-            if (P.relu) {
-#pragma unroll
-              for (int k = 0; k < 16; ++k) g[k] = fmaxf(g[k], 0.f);
-            }
-            if (P.out_fp32) {
-              float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(P.out) + pix * P.out_pix_stride + csoff);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) op[k] = make_float4(g[4 * k], g[4 * k + 1], g[4 * k + 2], g[4 * k + 3]);
-            } else {
-              uint32_t pk[8];
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                __nv_bfloat162 h = __floats2bfloat162_rn(g[2 * k], g[2 * k + 1]);
-                pk[k] = *reinterpret_cast<uint32_t*>(&h);
-              }
-              uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(P.out) + pix * P.out_pix_stride + csoff);
-              op[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-              op[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-            }
-          }
-          __syncwarp();                                 // the transpose tile is rewritten by the next chunk
-        }
-        stx += 16;
-        while (stx >= P.TW) { stx -= P.TW; ++sty; }
+        for (int k = 0; k < BLOCK_K / 16; ++k)   // 16 bf16 = 32 bytes along K inside the swizzle span: +2 in (addr>>4)
+          ptx::wgmma_bf16<BLOCK_N, 0, 0>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<1>();                    // the previous K block's MMAs are done: its slot can be refilled
+        if (prev >= 0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty_bar[prev]); }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      // the accumulator has been read: hand it back to the MMA warp before the statistics hand-shake
-      ptx::tcgen05_fence_before();
+      ptx::wgmma_wait<0>();
+      ptx::fence_regs(acc);
       __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      if (P.stats) {
-        // the two halves of a channel: upper half -> shared memory -> lower half adds (fixed order) and writes the tile's row
-        if (half == 1) { sstat[co] = ssum; sstat[128 + co] = ssq; }
-        ptx::named_bar_sync(1 + q, 64);
-        if (half == 0 && cvalid) {
-          float* dst = P.stats + (size_t)tile * 2 * P.Cout;
-          dst[co] = ssum + sstat[co]; dst[P.Cout + co] = ssq + sstat[128 + co];
-        }
-        ptx::named_bar_sync(1 + q, 64);                 // sstat is rewritten by the next tile
-      }
+      if (lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+      conv_epilogue_tile<BLOCK_N>(P, acc, warp, lane, img, th_i * P.TH, tw_i * P.TW, n0, tile_m, red);
     }
   }
-  ptx::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tcgen05_fence_after();
-    ptx::tmem_dealloc<512>(tmem_base);
-  }
-}
-
-// 256-pixel tile for the swapped kernel
-static double pick_tile256(int Ho, int Wo, int stride, int* TH, int* TW) {
-  double best = -1; int bth = 1, btw = 1;
-  for (int tw = 1; tw <= 256 && tw <= Wo; ++tw) {
-    if (tw * stride > 256) break;
-    int th = 256 / tw; if (th > Ho) th = Ho;
-    if (th * stride > 256) th = 256 / stride;
-    if (th < 1) continue;
-    long long tiles = (long long)((Ho + th - 1) / th) * ((Wo + tw - 1) / tw);
-    double eff = (double)Ho * Wo / (double)(tiles * 256);
-    if (eff > best + 1e-9 || (eff > best - 1e-9 && tw > btw)) { best = eff; bth = th; btw = tw; }
-  }
-  *TH = bth; *TW = btw;
-  return best;
 }
 
 // ---- host side --------------------------------------------------------------------------------
@@ -661,30 +254,35 @@ static void pick_tile(int Ho, int Wo, int stride, int* TH, int* TW) {
   *TH = bth; *TW = btw;
 }
 
-template <int BN, int BK, int ST>
-static int32_t launch_conv(const CUtensorMap& mx, const CUtensorMap& mw, const ConvKParams& P, dim3 grid,
+template <int BN, int BK, int ST, int CPS>
+static int32_t launch_conv(const CUtensorMap& mx, const CUtensorMap& mw, const ConvKParams& P, int tiles_m, int n_tiles,
                            cudaStream_t st) {
   using S = ConvSmem<BN, BK, ST>;
-  auto kern = conv_tc_kernel<BN, BK, ST>;
+  static_assert(CPS * (S::kTotal + 1024) <= 228 * 1024, "conv: shared memory of CPS CTAs exceeds the SM");
+  auto kern = conv_tc_kernel<BN, BK, ST, CPS>;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
     if (e != cudaSuccess) return set_error(C3D_ECUDA, "conv smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
-  kern<<<grid, 192, S::kTotal, st>>>(mx, mw, P);
+  long long total = (long long)tiles_m * n_tiles;
+  long long grid = (long long)kNumSMs * CPS;
+  if (grid > total) grid = total;
+  kern<<<(unsigned)grid, kGemmThreads, S::kTotal, st>>>(mx, mw, P, tiles_m, n_tiles);
   return check_launch("conv_tc_kernel");
 }
 
 
 // ------------------------------------------------------------------------------------------------
 // Weight gradient: dW[co][kh][kw][ci] += sum_pixels dY[p][co] * X[p*stride + tap - pad][ci].
-// GEMM view: M = Cout (128 per CTA), N = (tap, ci) columns — up to 256 per CTA, made of whole TMA boxes
-// [pixels][cw channels] (cw = 64/32/16), so small-Cin layers put SEVERAL TAPS side by side in N and dY is
-// re-read ceil(taps*Cin/256) times instead of `taps` times — K = pixels.  Both operands are "MN-major"
-// for the tensor core (the contiguous NHWC channel axis is M resp. N, pixels are K): the same 4-D TMA
-// boxes as the forward pass are consumed through MN-major shared-memory descriptors.  Grid = (pixel-range
-// split, column group, co tile); split-K partials are reduced with fp32 atomics into the gradient buffer.
+// GEMM view: M = Cout (128 per CTA: 64 per consumer warpgroup), N = (tap, ci) columns — up to 256 per CTA, made of
+// whole TMA boxes [pixels][cw channels] (cw = 64/32/16), so small-Cin layers put SEVERAL TAPS side by side in N and dY
+// is re-read ceil(taps*Cin/256) times instead of `taps` times — K = pixels.  Both operands are "MN-major" for the
+// tensor core (the contiguous NHWC channel axis is M resp. N, pixels are K): the same 4-D TMA boxes as the forward pass
+// are consumed through transposed wgmma descriptors.  Grid = (pixel-range split, column group, co tile); split-K
+// partials are stored per split and summed in split order by wgrad_reduce_kernel, so the result does not depend on the
+// order in which CTAs finish.
 struct WgradKParams {
   int N, Ho, Wo, Cout, Cin;
   int KH, KW, stride, pad;
@@ -692,103 +290,182 @@ struct WgradKParams {
   int num_tiles, tiles_per_split;
   int cw, nci, boxes_per_cta, total_boxes;   // B boxes: width cw channels, nci = Cin / cw per tap
   int ca, a_chunks_max;                      // A boxes: width ca channels
-  float* dw;                                 // fp32, accumulated with atomics
+  float* dw;                                 // fp32 gradient (+=), or null when `part` is set
+  float* part;                               // split-K partials [splits][welems] (plain stores), reduced in split order
+  long long welems;
   int oihw;                                  // 0: dw is [Cout][KH][KW][Cin]; 1: [Cout][Cin][KH][KW] (master layout)
   int big, mc;                               // 1: 5-D tensor maps — ONE box carries all channel chunks of dY (and mc chunks of X)
-  int dbg;                                   // lab switches (C3D_WGRAD_DBG): 1 no MMA, 2 no TMA, 4 no B loads, 8 no A loads
   int lin;                                   // 1: fully-connected layer (c3d_linear_wgrad): x is (rows, KH*KW*Cin) with the
                                              // features in (tap, ci) order — box b reads channels [b*cw, (b+1)*cw) with no
                                              // spatial shift; KH/KW/Cin only drive the epilogue's master-layout index
 };
 
-// PIX = pixels (GEMM K) per pipeline stage: 128 px x 2 stages or 64 px x 4 stages (same 192 KB).  The deeper pipeline
-// hides the TMA latency (a 128-px stage is only ~0.5 us of MMA work, less than one L2/HBM round trip), the larger
-// box fits feature maps whose rows do not tile into 64-pixel boxes (20x20 -> 4x20).
-template <int STAGES, int PIX, int NCOLS = 256, int MT = 1>
+// PIX = pixels (GEMM K) per pipeline stage: 128 px x 2 stages or 64 px x 4 stages (same 192 KB).  The larger box fits
+// feature maps whose rows do not tile into 64-pixel boxes (20x20 -> 4x20).
+template <int STAGES, int PIX, int NCOLS = 256>
 struct WgradSmem {
-  static constexpr int kABytes = PIX * 128 * MT * 2;       // MT x (up to two [PIX px][64 ch] chunks (or narrower))
+  static constexpr int kABytes = PIX * 128 * 2;            // up to two [PIX px][64 ch] chunks (or narrower)
   static constexpr int kBBytes = PIX * NCOLS * 2;          // NCOLS columns x PIX pixels
   static constexpr int kStageBytes = kABytes + kBBytes;    // 96 KB (PIX 128) / 48 KB (PIX 64)
   static constexpr int kBarOffset = STAGES * kStageBytes;
   static constexpr int kTotal = kBarOffset + 256 + 1024;
 };
 
-// MT = 128-row output-channel tiles per CTA: with MT = 2 one X tile feeds two accumulators (2 x 256 TMEM columns), so a
-// stage moves 64 KB for 2 x 4 MMAs instead of 96 KB for 8 — a third less L2 -> SM traffic per FLOP (the L2 port, ~42 B/clk/SM,
-// is what bounds this loop) and three pipeline stages instead of two.
-template <int STAGES, int PIX, int NCOLS = 256, int MT = 1>
-__global__ void __launch_bounds__(192)
+// main loop + epilogue of one consumer warpgroup with an NB-column accumulator (NB >= the CTA's columns rounded up to
+// 64; the extra columns read stale shared memory and are never stored)
+template <int NB, int STAGES, int PIX, int NCOLS>
+__device__ __forceinline__ void wgrad_consume(const WgradKParams& P, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                              const int t_begin, const int t_end, const int warp, const int lane,
+                                              const int co0, const int box0, const int ncols, const uint32_t a_box_bytes,
+                                              const uint32_t b_box_bytes) {
+  using S = WgradSmem<STAGES, PIX, NCOLS>;
+  const int wg = warp >> 2;
+  const bool active = co0 + wg * 64 < P.Cout;        // this warpgroup's 64 output channels exist
+  float acc[NB / 2];
+#pragma unroll
+  for (int i = 0; i < NB / 2; ++i) acc[i] = 0.f;
+  const uint32_t lt_a = ptx::swizzle_layout_type(P.ca * 2), lt_b = ptx::swizzle_layout_type(P.cw * 2);
+  const int ksteps = (P.RH * P.RW) / 16;
+  // MN-major descriptors: LBO = distance between channel chunks, SBO = 8 pixel rows
+  const uint32_t a_sbo = 8 * P.ca * 2, b_sbo = 8 * P.cw * 2;
+  const uint32_t a_kstep = (16 * P.ca * 2) >> 4, b_kstep = (16 * P.cw * 2) >> 4;
+  const uint32_t a_off = (uint32_t)(wg * (64 / P.ca)) * a_box_bytes;   // first dY chunk of this warpgroup's channels
+  int stage = 0; uint32_t phase = 0;
+  int prev = -1;
+  for (int t = t_begin; t < t_end; ++t) {
+    ptx::mbar_wait(&full_bar[stage], phase);
+    if (active) {
+      const uint32_t sa = ptx::smem_u32(smem + stage * S::kStageBytes);
+      const uint64_t da = ptx::make_smem_desc(sa + a_off, a_box_bytes, a_sbo, lt_a);
+      const uint64_t db = ptx::make_smem_desc(sa + S::kABytes, b_box_bytes, b_sbo, lt_b);
+      ptx::wgmma_fence();
+      for (int k = 0; k < ksteps; ++k)
+        ptx::wgmma_bf16<NB, 1, 1>(acc, da + (uint64_t)(a_kstep * k), db + (uint64_t)(b_kstep * k), 1u);
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<1>();
+    }
+    if (prev >= 0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty_bar[prev]); }
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(acc);
+  __syncwarp();
+  if (lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+  if (!active) return;
+  const int taps = P.KH * P.KW;
+#pragma unroll
+  for (int j = 0; j < NB / 8; ++j) {
+    const int n = 8 * j + 2 * (lane & 3);             // column pair (n, n + 1): same box, consecutive ci
+    if (n >= ncols) continue;
+    const int box = box0 + n / P.cw;
+    const int tap = box / P.nci, ci = (box - tap * P.nci) * P.cw + (n % P.cw);
+    if (ci >= P.Cin) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int co = co0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      if (co >= P.Cout) continue;
+      const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      // one writer per element: a plain store of this split's partial, or (single split) dw +=
+      float* base = P.part ? P.part + (size_t)blockIdx.x * P.welems : P.dw;
+      if (P.oihw) {
+        float* dst = base + ((size_t)co * P.Cin + ci) * taps + tap;
+        if (P.part) { dst[0] = v0; dst[taps] = v1; } else { dst[0] += v0; dst[taps] += v1; }
+      } else {
+        float2* dst = reinterpret_cast<float2*>(base + ((size_t)co * taps + tap) * P.Cin + ci);
+        if (P.part) *dst = make_float2(v0, v1);
+        else { float2 o = *dst; o.x += v0; o.y += v1; *dst = o; }
+      }
+    }
+  }
+}
+
+// dw[e] += sum over s of part[s][e], summed in s order (deterministic split-K reduction)
+__global__ void wgrad_reduce_kernel(const float* __restrict__ part, int nparts, long long welems, float* __restrict__ dw) {
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < welems; e += (long long)gridDim.x * blockDim.x) {
+    float a = 0.f;
+    for (int s = 0; s < nparts; ++s) a += part[(size_t)s * welems + e];
+    dw[e] += a;
+  }
+}
+// runs `launch(part)` with a stream-ordered partial buffer of nparts x welems floats (null when nparts == 1: the kernel
+// then adds into dw itself), then reduces the partials into dw in a fixed order
+template <typename F>
+static int32_t with_ordered_partials(int nparts, long long welems, float* dw, cudaStream_t st, F launch) {
+  if (nparts <= 1) return launch(nullptr);
+  float* part = nullptr;
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&part), (size_t)nparts * welems * sizeof(float), st);
+  if (e != cudaSuccess) return set_error(C3D_ECUDA, "wgrad partials: %s", cudaGetErrorString(e));
+  int32_t rc = launch(part);
+  if (rc == C3D_OK) {
+    long long blocks = (welems + 255) / 256;
+    if (blocks > 8LL * kNumSMs) blocks = 8LL * kNumSMs;
+    wgrad_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, nparts, welems, dw);
+    rc = check_launch("wgrad_reduce_kernel");
+  }
+  e = cudaFreeAsync(part, st);
+  if (rc == C3D_OK && e != cudaSuccess) rc = set_error(C3D_ECUDA, "wgrad partials free: %s", cudaGetErrorString(e));
+  return rc;
+}
+
+template <int STAGES, int PIX, int NCOLS = 256>
+__global__ void __launch_bounds__(kGemmThreads, 1)
 conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
                      const WgradKParams P) {
-  using S = WgradSmem<STAGES, PIX, NCOLS, MT>;
+  using S = WgradSmem<STAGES, PIX, NCOLS>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   const int split = blockIdx.x, group = blockIdx.y, co_tile = blockIdx.z;
-  const int co0 = co_tile * 128 * MT;
+  const int co0 = co_tile * 128;
   const int box0 = group * P.boxes_per_cta;
   const int nb = min(P.boxes_per_cta, P.total_boxes - box0);       // boxes (taps x ci chunks) of this CTA
-  const int ncols = nb * P.cw;                                     // UMMA N (multiple of 16, <= 256)
+  const int ncols = nb * P.cw;                                     // GEMM N (multiple of 16, <= NCOLS)
   const int t_begin = split * P.tiles_per_split;
   const int t_end = min(P.num_tiles, t_begin + P.tiles_per_split);
+  if (t_begin >= t_end) return;
   const int R = P.RH * P.RW;
   int a_chunks = (P.Cout - co0 + P.ca - 1) / P.ca;
   if (a_chunks > P.a_chunks_max) a_chunks = P.a_chunks_max;
   // distance between channel chunks in shared memory: a full PIX-pixel slot per box, or (5-D boxes) the dense box pitch
   const uint32_t a_box_bytes = (uint32_t)((P.big ? R : PIX) * P.ca * 2), b_box_bytes = (uint32_t)((P.big ? R : PIX) * P.cw * 2);
 
-  if (warp == 0 && lane == 0) { ptx::prefetch_tensormap(&tmap_dy); ptx::prefetch_tensormap(&tmap_x); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], 1); }
-    ptx::mbar_init(tmem_full_bar, 1);
+  if (warp == kConsumerWarps && lane == 0) {
+    ptx::prefetch_tensormap(&tmap_dy); ptx::prefetch_tensormap(&tmap_x);
+    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kConsumerWarps); }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) ptx::tmem_alloc<256 * MT>(tmem_ptr);
-  ptx::tcgen05_fence_before();
   __syncthreads();
-  ptx::tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (t_begin < t_end) {
-    if (warp == 0) {
-      if (ptx::elect_one()) {
-        int stage = 0; uint32_t phase = 0;
-        uint32_t bytes = (uint32_t)(R * 2 * ((P.big ? P.a_chunks_max : a_chunks) * P.ca + nb * P.cw));
-        if C3D_DBG(P, 4) bytes = (uint32_t)(R * 2 * (a_chunks * P.ca));
-        if C3D_DBG(P, 8) bytes = (uint32_t)(R * 2 * (nb * P.cw));
-        for (int t = t_begin; t < t_end; ++t) {
-          const int tw_i = t % P.tiles_w, th_i = (t / P.tiles_w) % P.tiles_h, img = t / (P.tiles_w * P.tiles_h);
-          const int ho0 = th_i * P.RH, wo0 = tw_i * P.RW;
-          ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * S::kStageBytes;
-          uint8_t* sb = sa + S::kABytes;
-          if C3D_DBG(P, 2) { ptx::mbar_arrive(&full_bar[stage]); if (++stage == STAGES) { stage = 0; phase ^= 1; } continue; }
-          ptx::mbar_expect_tx(&full_bar[stage], bytes);
-          if (P.big) {
-            if (!C3D_DBG(P, 8)) ptx::tma_load_5d(sa, &tmap_dy, &full_bar[stage], 0, wo0, ho0, co0 / P.ca, img);
-            if (!C3D_DBG(P, 4))
-            for (int b = 0; b < nb; b += P.mc) {
-              const int box = box0 + b;
-              const int tap = box / P.nci, chunk = box - tap * P.nci;
-              const int kh = tap / P.KW, kw = tap - kh * P.KW;
-              if (P.lin)
-                ptx::tma_load_5d(sb + b * b_box_bytes, &tmap_x, &full_bar[stage], 0, wo0, ho0, box, img);
-              else
-                ptx::tma_load_5d(sb + b * b_box_bytes, &tmap_x, &full_bar[stage], 0, wo0 * P.stride + kw - P.pad,
-                                 ho0 * P.stride + kh - P.pad, chunk, img);
-            }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            continue;
+  if (warp == kConsumerWarps) {
+    if (ptx::elect_one()) {
+      int stage = 0; uint32_t phase = 0;
+      const uint32_t bytes = (uint32_t)(R * 2 * ((P.big ? P.a_chunks_max : a_chunks) * P.ca + nb * P.cw));
+      for (int t = t_begin; t < t_end; ++t) {
+        const int tw_i = t % P.tiles_w, th_i = (t / P.tiles_w) % P.tiles_h, img = t / (P.tiles_w * P.tiles_h);
+        const int ho0 = th_i * P.RH, wo0 = tw_i * P.RW;
+        ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sa = smem + stage * S::kStageBytes;
+        uint8_t* sb = sa + S::kABytes;
+        ptx::mbar_expect_tx(&full_bar[stage], bytes);
+        if (P.big) {
+          ptx::tma_load_5d(sa, &tmap_dy, &full_bar[stage], 0, wo0, ho0, co0 / P.ca, img);
+          for (int b = 0; b < nb; b += P.mc) {
+            const int box = box0 + b;
+            const int tap = box / P.nci, chunk = box - tap * P.nci;
+            const int kh = tap / P.KW, kw = tap - kh * P.KW;
+            if (P.lin)
+              ptx::tma_load_5d(sb + b * b_box_bytes, &tmap_x, &full_bar[stage], 0, wo0, ho0, box, img);
+            else
+              ptx::tma_load_5d(sb + b * b_box_bytes, &tmap_x, &full_bar[stage], 0, wo0 * P.stride + kw - P.pad,
+                               ho0 * P.stride + kh - P.pad, chunk, img);
           }
-          if (!C3D_DBG(P, 8))
+        } else {
           for (int c = 0; c < a_chunks; ++c)
             ptx::tma_load_4d(sa + c * a_box_bytes, &tmap_dy, &full_bar[stage], co0 + P.ca * c, wo0, ho0, img);
-          if (!C3D_DBG(P, 4))
           for (int b = 0; b < nb; ++b) {
             const int box = box0 + b;
             const int tap = box / P.nci, chunk = box - tap * P.nci;
@@ -799,80 +476,23 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
               ptx::tma_load_4d(sb + b * b_box_bytes, &tmap_x, &full_bar[stage], chunk * P.cw,
                                wo0 * P.stride + kw - P.pad, ho0 * P.stride + kh - P.pad, img);
           }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-      }
-    } else if (warp == 1) {
-      if (ptx::elect_one()) {
-        const uint32_t idesc = ptx::make_idesc_bf16(128, ncols, 1, 1);
-        const uint32_t lt_a = ptx::swizzle_layout_type(P.ca * 2), lt_b = ptx::swizzle_layout_type(P.cw * 2);
-        int stage = 0; uint32_t phase = 0;
-        const int ksteps = R / 16;
-        // MN-major descriptors: LBO = distance between channel chunks, SBO = 8 pixel rows
-        const uint32_t a_sbo = 8 * P.ca * 2, b_sbo = 8 * P.cw * 2;
-        const uint32_t a_kstep = (16 * P.ca * 2) >> 4, b_kstep = (16 * P.cw * 2) >> 4;
-        for (int t = t_begin; t < t_end; ++t) {
-          ptx::mbar_wait(&full_bar[stage], phase);
-          if C3D_DBG(P, 1) { ptx::mbar_arrive(&empty_bar[stage]); if (++stage == STAGES) { stage = 0; phase ^= 1; } continue; }
-          ptx::tcgen05_fence_after();
-          const uint32_t sa = ptx::smem_u32(smem + stage * S::kStageBytes);
-          const uint32_t sb = sa + S::kABytes;
-          const uint64_t da = ptx::make_smem_desc(sa, a_box_bytes, a_sbo, lt_a);
-          const uint64_t db = ptx::make_smem_desc(sb, b_box_bytes, b_sbo, lt_b);
-#pragma unroll
-          for (int m = 0; m < MT; ++m) {
-            // output-channel tile m = chunks [m * 128 / ca, (m + 1) * 128 / ca) of the dY box
-            const uint64_t dam = da + (uint64_t)((m * (128 / P.ca) * a_box_bytes) >> 4);
-            for (int k = 0; k < ksteps; ++k)
-              ptx::umma_bf16(tmem_base + (uint32_t)(m * 256), dam + (uint64_t)(a_kstep * k), db + (uint64_t)(b_kstep * k), idesc,
-                             (t != t_begin || k != 0) ? 1u : 0u);
-          }
-          ptx::umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        ptx::umma_commit(tmem_full_bar);
-      }
-    } else {
-      const int q = warp & 3;
-      ptx::mbar_wait(tmem_full_bar, 0);
-      ptx::tcgen05_fence_after();
-      const int taps = P.KH * P.KW;
-#pragma unroll 1
-      for (int mch = 0; mch * 16 < ncols * MT; ++mch) {
-        const int m = MT == 1 ? 0 : (mch * 16) / ncols, ch = mch - m * (ncols / 16);
-        const int co = co0 + m * 128 + q * 32 + lane;
-        uint32_t v[16];
-        ptx::tmem_ld_32x32b_x16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(m * 256 + ch * 16), v);
-        ptx::tmem_ld_wait();
-        const int n = ch * 16;
-        const int box = box0 + n / P.cw;
-        const int tap = box / P.nci, ci = (box - tap * P.nci) * P.cw + (n % P.cw);
-        if (co < P.Cout && ci < P.Cin) {
-          const int lim = min(16, P.Cin - ci);
-          if (P.oihw) {
-            float* dst = P.dw + ((size_t)co * P.Cin + ci) * taps + tap;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) if (i < lim) atomicAdd(dst + (size_t)i * taps, __uint_as_float(v[i]));
-          } else {
-            float4* dst = reinterpret_cast<float4*>(P.dw + ((size_t)co * taps + tap) * P.Cin + ci);   // 64-B aligned
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              atomicAdd(dst + i, make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]),
-                                             __uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3])));
-          }
-        }
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  }
-  ptx::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tcgen05_fence_after();
-    ptx::tmem_dealloc<256 * MT>(tmem_base);
+  } else {
+    if (NCOLS > 192 && ncols > 192)
+      wgrad_consume<(NCOLS > 192 ? 256 : 64), STAGES, PIX, NCOLS>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
+    else if (NCOLS > 128 && ncols > 128)
+      wgrad_consume<(NCOLS > 128 ? 192 : 64), STAGES, PIX, NCOLS>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
+    else if (ncols > 64)
+      wgrad_consume<128, STAGES, PIX, NCOLS>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
+    else
+      wgrad_consume<64, STAGES, PIX, NCOLS>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
   }
 }
 
-// pixel box for wgrad: RH*RW must be a multiple of 16 (UMMA K) and <= max_pix; returns the covered fraction
+// pixel box for wgrad: RH*RW must be a multiple of 16 (wgmma K) and <= max_pix; returns the covered fraction
 static double pick_tile_k(int Ho, int Wo, int stride, int* RH, int* RW, int max_pix = 128) {
   double best = -1; int bth = 1, btw = 16;
   for (int tw = 1; tw <= max_pix; ++tw) {
@@ -889,51 +509,11 @@ static double pick_tile_k(int Ho, int Wo, int stride, int* RH, int* RW, int max_
   return best;
 }
 
-template <int BN, int BK, int ST>
-static int32_t launch_conv_p(const CUtensorMap& mx, const CUtensorMap& mw, const ConvKParams& P, int tiles_m, int n_tiles,
-                             int ctas_per_sm, cudaStream_t st) {
-  using S = ConvSmem<BN, BK, ST>;
-  auto kern = conv_tc_persistent_kernel<BN, BK, ST>;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
-    if (e != cudaSuccess) return set_error(C3D_ECUDA, "conv smem attr: %s", cudaGetErrorString(e));
-    attr = true;
-  }
-  long long total = (long long)tiles_m * n_tiles;
-  long long grid = (long long)kNumSMs * ctas_per_sm;
-  if (grid > total) grid = total;
-  kern<<<(unsigned)grid, 192, S::kTotal, st>>>(mx, mw, P, tiles_m, n_tiles);
-  return check_launch("conv_tc_persistent_kernel");
-}
-
 }  // namespace c3d
 
 #include "conv_halo.cuh"
 
 using namespace c3d;
-
-// swapped (Cout-as-M) kernel: 64 or 128 output channels, 64-deep K blocks, the layers the persistent kernel takes
-static bool swap_fwd_eligible(const c3d_conv_desc* d, int Ho, int Wo, int* th, int* tw) {
-  static const bool off = getenv("C3D_CONV_NO_SWAP") != nullptr || getenv("C3D_CONV_NONPERSISTENT") != nullptr;
-  if (off || halo_fwd_eligible(d)) return false;
-  if (d->Cin % 64 != 0 || (d->Cout != 64 && d->Cout != 128) || (d->KH == 1 && d->Cin <= 64)) return false;
-  if (d->stride < 1 || d->stride > 2) return false;
-  if (d->Cout == 64) {
-    // 64 output channels use half of the TMEM lanes, i.e. half of the epilogue warps: a win only when a tile carries enough
-    // MMA work per stored pixel (3x3: 9 K blocks) or the layer is a large HBM-bound 1x1 (measured, profiles/r02_summary.md);
-    // the phase convs of a stride-2 data gradient (1..4 taps) and small 1x1 layers stay on the pixel-major kernels
-    const long long num_kb = (long long)d->KH * d->KW * (d->Cin / 64);
-    const bool big_1x1 = d->KH == 1 && d->KW == 1 && (long long)d->N * Ho * Wo >= (1ll << 19);
-    if (num_kb < 9 && !big_1x1) return false;
-  }
-  int th128, tw128;
-  pick_tile(Ho, Wo, d->stride, &th128, &tw128);
-  const long long t128 = (long long)((Ho + th128 - 1) / th128) * ((Wo + tw128 - 1) / tw128);
-  const double eff128 = (double)Ho * Wo / (double)(t128 * 128);
-  const double eff256 = pick_tile256(Ho, Wo, d->stride, th, tw);
-  return eff256 >= 0.85 * eff128;
-}
 
 extern "C" int32_t c3d_conv2d_tiles(const c3d_conv_desc* d, int32_t* tiles_m, int32_t* TH, int32_t* TW) {
   if (!d) return set_error(C3D_EINVAL, "null desc");
@@ -946,7 +526,7 @@ extern "C" int32_t c3d_conv2d_tiles(const c3d_conv_desc* d, int32_t* tiles_m, in
     return C3D_OK;
   }
   int th, tw;
-  if (!swap_fwd_eligible(d, Ho, Wo, &th, &tw)) pick_tile(Ho, Wo, d->stride, &th, &tw);
+  pick_tile(Ho, Wo, d->stride, &th, &tw);
   if (TH) *TH = th;
   if (TW) *TW = tw;
   if (tiles_m) *tiles_m = d->N * ((Ho + th - 1) / th) * ((Wo + tw - 1) / tw);
@@ -962,15 +542,11 @@ extern "C" int32_t c3d_conv2d_fwd(const c3d_conv_desc* d, const void* x, const v
   if (Cout % 16 != 0 || Cout <= 0) return set_error(C3D_EINVAL, "conv2d: Cout=%d must be a multiple of 16", Cout);
   if (d->stride < 1 || d->stride > 2) return set_error(C3D_EINVAL, "conv2d: stride %d unsupported", d->stride);
   const int BK = (Cin % 64 == 0) ? 64 : (Cin % 32 == 0 ? 32 : 16);
-  static const bool non_persistent = getenv("C3D_CONV_NONPERSISTENT") != nullptr;
-  static const bool allow_n256 = getenv("C3D_CONV_NO_N256") == nullptr;
   int BN = 128;
   if (Cout % 128 != 0) BN = (Cout % 64 == 0) ? 64 : (Cout % 32 == 0 ? 32 : 16);
-  // persistent + double-buffered TMEM pays off for the tensor-bound shapes; the tiny-K / memory-bound ones
-  // (Cin < 64, or 1x1 with Cin <= 64) run better as many short CTAs (measured, profiles/)
-  static const bool p1x1 = getenv("C3D_CONV_P1X1") != nullptr;      // lab: one-K-block 1x1 layers on the persistent kernel
-  const bool persistent = !non_persistent && BK == 64 && BN >= 64 && (p1x1 || !(d->KH == 1 && Cin <= 64));
-  if (persistent && allow_n256 && Cout % 256 == 0) BN = 256;
+  // N = 256 (one CTA per SM, 128 accumulator registers per thread) for the layers with several 64-deep K blocks; the
+  // 1x1 layers over <= 64 channels are memory-bound and keep two CTAs per SM
+  if (BK == 64 && !(d->KH == 1 && Cin <= 64) && Cout % 256 == 0) BN = 256;
   const int Ho = d->out_h > 0 ? d->out_h : (d->H + 2 * d->pad - d->KH) / d->stride + 1;
   const int Wo = d->out_w > 0 ? d->out_w : (d->W + 2 * d->pad - d->KW) / d->stride + 1;
   if (d->add_mode == 2 && ((Ho & 1) || (Wo & 1))) return set_error(C3D_EINVAL, "conv2d: up2 addend needs even output");
@@ -984,13 +560,7 @@ extern "C" int32_t c3d_conv2d_fwd(const c3d_conv_desc* d, const void* x, const v
 
   ConvKParams P;
   P.N = d->N; P.Ho = Ho; P.Wo = Wo; P.Cout = Cout; P.KH = d->KH; P.KW = d->KW; P.stride = d->stride; P.pad = d->pad;
-  P.dbg = 0;
-#ifdef C3D_LAB
-  { const char* e = getenv("C3D_CONV_DBG"); P.dbg = e ? atoi(e) : 0; }
-#endif
-  const bool swap = swap_fwd_eligible(d, Ho, Wo, &P.TH, &P.TW);
-  if (swap) BN = Cout;                                   // weight box rows
-  else pick_tile(Ho, Wo, d->stride, &P.TH, &P.TW);
+  pick_tile(Ho, Wo, d->stride, &P.TH, &P.TW);
   P.tiles_h = (Ho + P.TH - 1) / P.TH; P.tiles_w = (Wo + P.TW - 1) / P.TW;
   P.kc_blocks = Cin / BK; P.Cin = Cin;
   P.bias = bias; P.relu = d->relu; P.out_fp32 = d->out_fp32; P.add_mode = d->add_mode;
@@ -1029,61 +599,25 @@ extern "C" int32_t c3d_conv2d_fwd(const c3d_conv_desc* d, const void* x, const v
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return set_error(C3D_ECUDA, "encode w tensormap failed: %d", (int)r);
   }
-  dim3 grid((unsigned)(d->N * P.tiles_h * P.tiles_w), (unsigned)(Cout / BN));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (swap) {
-    static bool attr = false;
-    if (!attr) {
-      cudaError_t e = cudaFuncSetAttribute(conv_tc_swap_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ConvSwapSmem::kTotal);
-      if (e != cudaSuccess) return set_error(C3D_ECUDA, "conv swap smem attr: %s", cudaGetErrorString(e));
-      attr = true;
-    }
-    const int tiles_m = d->N * P.tiles_h * P.tiles_w;
-    conv_tc_swap_kernel<<<(unsigned)(tiles_m < kNumSMs ? tiles_m : kNumSMs), ConvSwapSmem::kThreads, ConvSwapSmem::kTotal, st>>>(mx, mw, P, tiles_m);
-    return check_launch("conv_tc_swap_kernel");
-  }
-  if (persistent) {
-    const int tiles_m = d->N * P.tiles_h * P.tiles_w, n_tiles = Cout / BN;
-#define C3D_CONV_P(bn, bk, stg, cps) \
-    if (BN == bn && BK == bk) return launch_conv_p<bn, bk, stg>(mx, mw, P, tiles_m, n_tiles, cps, st);
-    C3D_CONV_P(256, 64, 4, 1)
-    C3D_CONV_P(128, 64, 6, 1)
-    C3D_CONV_P(64, 64, 8, 1)
-    C3D_CONV_P(32, 64, 8, 1)
-    C3D_CONV_P(16, 64, 8, 1)
-    C3D_CONV_P(128, 32, 8, 1)
-    C3D_CONV_P(64, 32, 8, 2)
-    C3D_CONV_P(32, 32, 8, 2)
-    C3D_CONV_P(16, 32, 8, 2)
-    C3D_CONV_P(128, 16, 8, 2)
-    C3D_CONV_P(64, 16, 8, 2)
-    C3D_CONV_P(32, 16, 8, 4)
-    C3D_CONV_P(16, 16, 8, 4)
-#undef C3D_CONV_P
-  }
-#define C3D_CONV_CASE(bn, bk, stg) \
-  if (BN == bn && BK == bk) return launch_conv<bn, bk, stg>(mx, mw, P, grid, st);
-  // one K block per tile (1x1 convs with Cin <= 64: FPN lateral 64->256, DLA projections): these CTAs live for one
-  // TMA -> MMA -> epilogue round trip (~7 us, ncu) and the layer is bound by how many of them an SM holds — a single
-  // pipeline stage (35 KB instead of 99 KB of shared memory) lets the 512 TMEM columns, not shared memory, set the limit
-  if (d->KH * d->KW * P.kc_blocks == 1) {
-    C3D_CONV_CASE(128, 64, 1)
-    C3D_CONV_CASE(64, 64, 1)
-    C3D_CONV_CASE(128, 32, 1)
-    C3D_CONV_CASE(64, 32, 1)
-  }
-  C3D_CONV_CASE(128, 64, 3)
-  C3D_CONV_CASE(64, 64, 4)
-  C3D_CONV_CASE(32, 64, 4)
-  C3D_CONV_CASE(16, 64, 4)
-  C3D_CONV_CASE(128, 32, 4)
-  C3D_CONV_CASE(64, 32, 4)
-  C3D_CONV_CASE(32, 32, 4)
-  C3D_CONV_CASE(16, 32, 4)
-  C3D_CONV_CASE(128, 16, 4)
-  C3D_CONV_CASE(64, 16, 4)
-  C3D_CONV_CASE(32, 16, 4)
-  C3D_CONV_CASE(16, 16, 4)
+  const int tiles_m = d->N * P.tiles_h * P.tiles_w, n_tiles = Cout / BN;
+  // (BN, BK) -> pipeline stages, CTAs per SM: N = 256 fills the register file with one CTA; the others run two CTAs so
+  // that one CTA's epilogue overlaps the other's main loop
+#define C3D_CONV_CASE(bn, bk, stg, cps) \
+  if (BN == bn && BK == bk) return launch_conv<bn, bk, stg, cps>(mx, mw, P, tiles_m, n_tiles, st);
+  C3D_CONV_CASE(256, 64, 4, 1)
+  C3D_CONV_CASE(128, 64, 3, 2)
+  C3D_CONV_CASE(64, 64, 4, 2)
+  C3D_CONV_CASE(32, 64, 4, 2)
+  C3D_CONV_CASE(16, 64, 4, 2)
+  C3D_CONV_CASE(128, 32, 6, 2)
+  C3D_CONV_CASE(64, 32, 6, 2)
+  C3D_CONV_CASE(32, 32, 6, 2)
+  C3D_CONV_CASE(16, 32, 6, 2)
+  C3D_CONV_CASE(128, 16, 8, 2)
+  C3D_CONV_CASE(64, 16, 8, 2)
+  C3D_CONV_CASE(32, 16, 8, 2)
+  C3D_CONV_CASE(16, 16, 8, 2)
 #undef C3D_CONV_CASE
   return set_error(C3D_EINVAL, "conv2d: no kernel for BN=%d BK=%d", BN, BK);
 }
@@ -1117,10 +651,6 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   P.N = d->N; P.Ho = Ho; P.Wo = Wo; P.Cout = Cout; P.Cin = Cin;
   P.KH = d->KH; P.KW = d->KW; P.stride = d->stride; P.pad = d->pad;
   P.lin = lin_c > 0;
-  P.dbg = 0;
-#ifdef C3D_LAB
-  { const char* e = getenv("C3D_WGRAD_DBG"); P.dbg = e ? atoi(e) : 0; }
-#endif
   if (P.lin) {
     if (d->KH != 1 || d->KW != 1 || d->stride != 1 || d->pad != 0 || lin_c % 16 != 0 || (long long)lin_c * lin_pp != Cin)
       return set_error(C3D_EINVAL, "linear wgrad: bad feature factorisation %d x %d != %d", lin_c, lin_pp, Cin);
@@ -1130,17 +660,10 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   int rh64, rw64;
   const double eff128 = pick_tile_k(Ho, Wo, d->stride, &P.RH, &P.RW, 128);
   const double eff64 = pick_tile_k(Ho, Wo, d->stride, &rh64, &rw64, 64);
-  // measured (profiles/r02): the 4 x 64-pixel pipeline is SLOWER (fpn 3x3 @160: 0.92 -> 1.83 ms) — the loop is bound by the
-  // per-stage barrier round trip of the single MMA-issuing lane, not by TMA latency; kept as an opt-in experiment
+  // opt-in experiments: the 4 x 64-pixel pipeline, and 128 instead of 256 GEMM columns per CTA
   static const bool want64 = getenv("C3D_WGRAD_PIX64") != nullptr;
   static const bool n128 = getenv("C3D_WGRAD_N128") != nullptr;
-  static const bool no_mt2 = getenv("C3D_WGRAD_NO_MT2") != nullptr;
-  // two output-channel tiles per CTA (M = 256 through two accumulators) over 3 x 64-pixel stages: wide layers whose map tiles
-  // into 64-pixel boxes
-  // (not the small weight tensors below, <= 64K elements: those run ~4 waves of short CTAs and lose from halving the CTA count)
-  const bool mt2 = !no_mt2 && !n128 && Cout >= 256 && eff64 >= 0.93 * eff128 &&
-                   (long long)Cout * P.KH * P.KW * P.Cin > 65536;
-  const bool pix64 = mt2 || (want64 && eff64 >= 0.93 * eff128);
+  const bool pix64 = want64 && eff64 >= 0.93 * eff128;
   if (pix64) { P.RH = rh64; P.RW = rw64; }
   P.tiles_h = (Ho + P.RH - 1) / P.RH; P.tiles_w = (Wo + P.RW - 1) / P.RW;
   P.num_tiles = d->N * P.tiles_h * P.tiles_w;
@@ -1151,11 +674,11 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   P.boxes_per_cta = (n128 ? 128 : 256) / P.cw;
   P.total_boxes = taps * P.nci;
   P.ca = (Cout % 64 == 0) ? 64 : (Cout % 32 == 0 ? 32 : 16);
-  P.a_chunks_max = (mt2 ? 256 : 128) / P.ca;    // chunks beyond Cout are not loaded (those D rows are never stored)
+  P.a_chunks_max = 128 / P.ca;    // chunks beyond Cout are not loaded (those D rows are never stored)
   const int groups = (P.total_boxes + P.boxes_per_cta - 1) / P.boxes_per_cta;
-  const int co_tiles = mt2 ? (Cout + 255) / 256 : (Cout + 127) / 128;
-  // split-K over pixels (1 CTA/SM): every split costs 128 x N fp32 atomics, so big weight tensors get exactly one
-  // wave of CTAs (<= 148) while small ones (<= 64K elements: the pixel-heavy early layers) get ~4 waves for balance
+  const int co_tiles = (Cout + 127) / 128;
+  // split-K over pixels (1 CTA/SM): every split adds a 128 x N partial to the ordered reduction, so big weight tensors get exactly one
+  // wave of CTAs (<= kNumSMs) while small ones (<= 64K elements: the pixel-heavy early layers) get ~4 waves for balance
   long long base = (long long)groups * co_tiles;
   const long long welems = (long long)Cout * taps * Cin_e;
   int splits = welems <= 65536 ? (int)((4LL * kNumSMs + base - 1) / base) : (int)(kNumSMs / base);
@@ -1164,6 +687,8 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   P.tiles_per_split = (P.num_tiles + splits - 1) / splits;
   splits = (P.num_tiles + P.tiles_per_split - 1) / P.tiles_per_split;
   P.dw = dw;
+  P.part = nullptr;
+  P.welems = welems;
   P.oihw = oihw;
   const long long xps = d->x_pix_stride ? d->x_pix_stride : Cin;
   const long long yps = d->y_pix_stride ? d->y_pix_stride : Cout;
@@ -1172,7 +697,7 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   // with LBO = RH*RW*128 B — a third of the TMA instructions per stage (the loop is bound by boxes issued, not bytes)
   static const bool no_big = getenv("C3D_WGRAD_NO_BIGBOX") != nullptr;
   P.big = 0; P.mc = 1;
-  if (!no_big && !C3D_DBG(P, 12)) {
+  if (!no_big) {
     const int nchunks_x = P.lin ? P.total_boxes : P.nci;
     int mc = P.boxes_per_cta;
     while (mc > 1 && nchunks_x % mc != 0) mc >>= 1;
@@ -1233,22 +758,22 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
     if (e == cudaSuccess)
       e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<3, 128, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                WgradSmem<3, 128, 128>::kTotal);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<3, 64, 256, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               WgradSmem<3, 64, 256, 2>::kTotal);
     if (e != cudaSuccess) return set_error(C3D_ECUDA, "wgrad smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
-  if (mt2) conv_wgrad_tc_kernel<3, 64, 256, 2><<<grid, 192, WgradSmem<3, 64, 256, 2>::kTotal, st>>>(mdy, mx, P);
-  else if (n128 && !pix64) conv_wgrad_tc_kernel<3, 128, 128><<<grid, 192, WgradSmem<3, 128, 128>::kTotal, st>>>(mdy, mx, P);
-  else if (pix64) conv_wgrad_tc_kernel<4, 64><<<grid, 192, WgradSmem<4, 64>::kTotal, st>>>(mdy, mx, P);
-  else conv_wgrad_tc_kernel<2, 128><<<grid, 192, WgradSmem<2, 128>::kTotal, st>>>(mdy, mx, P);
-  return check_launch("conv_wgrad_tc_kernel");
+  return with_ordered_partials(splits, welems, dw, st, [&](float* part) -> int32_t {
+    WgradKParams Q = P;
+    Q.part = part;
+    if (n128 && !pix64) conv_wgrad_tc_kernel<3, 128, 128><<<grid, kGemmThreads, WgradSmem<3, 128, 128>::kTotal, st>>>(mdy, mx, Q);
+    else if (pix64) conv_wgrad_tc_kernel<4, 64><<<grid, kGemmThreads, WgradSmem<4, 64>::kTotal, st>>>(mdy, mx, Q);
+    else conv_wgrad_tc_kernel<2, 128><<<grid, kGemmThreads, WgradSmem<2, 128>::kTotal, st>>>(mdy, mx, Q);
+    return check_launch("conv_wgrad_tc_kernel");
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
 // Fully-connected layers of the box head / cube head (detectron2 FastRCNNConvFCHead, configs/Base.yaml:67-70;
-// cubercnn/modeling/roi_heads/cube_head.py:63-73,108-144) on the SAME tcgen05 kernels: a linear layer over `rows`
+// cubercnn/modeling/roi_heads/cube_head.py:63-73,108-144) on the SAME wgmma kernels: a linear layer over `rows`
 // feature vectors is the 1x1 convolution of a (1, 1, rows, K) "image" — 128-row M tiles, persistent CTAs, BLOCK_N 256,
 // bias + ReLU fused in the epilogue; the weight gradient is the split-K MN-major GEMM of conv_wgrad_tc_kernel.
 namespace c3d {

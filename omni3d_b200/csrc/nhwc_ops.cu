@@ -1,4 +1,4 @@
-// nhwc_ops.cu — HBM-bound NHWC bf16 kernels around the tensor-core convolutions (sm_100a):
+// nhwc_ops.cu — HBM-bound NHWC bf16 kernels around the tensor-core convolutions (sm_90a):
 // train-mode BatchNorm (finalize / apply+residual+ReLU / backward reduce+apply), 2x2 max-pool,
 // image normalisation + channel padding, fused SGD-momentum with finite check.
 //
@@ -7,7 +7,7 @@
 // GeneralizedRCNN.preprocess_image (called at rcnn3d.py:46,87) and the optimizer step +
 // per-parameter finite check (tools/train_net.py:226-252, cubercnn/solver/build.py:47-56).
 // All kernels: 16-byte vector loads (8 bf16 channels per thread), channel-innermost coalescing,
-// grid = multiple of 148 SMs with grid-stride loops; no tensor cores (byte work).
+// grid = multiple of the SM count with grid-stride loops; no tensor cores (byte work).
 #include <cuda_bf16.h>
 #include "c3d_common.cuh"
 
@@ -116,7 +116,7 @@ bn_apply_kernel(const bf16* __restrict__ y, const float* __restrict__ mean, cons
 // ---- BatchNorm backward -----------------------------------------------------------------------
 // dz = dout * (out > 0 if relu);  partial[block][0][c] = sum dz, partial[block][1][c] = sum dz * y  (the finalisation
 // turns the second sum into sum dz * xhat = rstd * (sum dz*y - mean * sum dz) in fp64).
-// Register diet (ncu / ptxas, profiles/r02): with mean / rstd / scale / shift / coefficients held per thread these kernels
+// Register diet (ptxas): with mean / rstd / scale / shift / coefficients held per thread these kernels
 // needed 86-90 registers => 2 CTAs of 256 threads per SM => too few loads in flight for HBM (they ran at ~60 % of the copy
 // bandwidth and got SLOWER when the ReLU-mask recomputation added 16 more).  Now the mask constants live in shared memory
 // (3 x C floats, read as two LDS.128 per array per pixel) and the arithmetic needs no per-channel constant at all (reduce) or
@@ -234,7 +234,7 @@ bn_bwd_apply_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ out,
 // ---- column sums + finalisation in ONE launch ------------------------------------------------------------------------
 // The three consumers of the slab sums (BatchNorm statistics, BatchNorm backward coefficients, bias gradient) used to be a
 // second launch of (C/32) tiny blocks behind colsum_stage1: ~100 extra launches of 5-10 us per step (1.2 ms with the
-// stage-1 kernels, profiles/r02).  Here the LAST stage-1 block to finish (ticket counter zeroed by a 4-byte memset node in
+// stage-1 kernels).  Here the LAST stage-1 block to finish (ticket counter zeroed by a 4-byte memset node in
 // front of the launch) runs the finalisation for all channels, in the same fixed order as before => same bits.
 struct FinArgs {
   int mode;                  // 0 BatchNorm statistics, 1 BatchNorm backward coefficients, 2 bias gradient

@@ -94,7 +94,7 @@ __device__ __forceinline__ int nms_scan_chunks(const unsigned long long* __restr
     cnt += __popcll(keep);
     // OR the kept rows' later words into the live bitset.  The rows are independent of each other: the loads of kUn kept rows
     // are issued before any of them is consumed (one kept row at a time was one L2 round trip per kept row — 1000 keeps x
-    // ~600 cycles = most of the 0.56 ms this kernel took per step, profiles/r02_summary.md)
+    // ~600 cycles per kept row)
     constexpr int kUn = 8;
     const bool w0 = lane > c && lane < wc, w1 = lane + 32 > c && lane + 32 < wc, w2 = lane + 64 > c && lane + 64 < wc,
                w3 = lane + 96 > c && lane + 96 < wc;

@@ -81,7 +81,8 @@ __global__ void __launch_bounds__(1024)
 topk_segments_kernel(const TopkParams P) {
   extern __shared__ unsigned long long sel[];            // [k2] (key << 32 | ~index)
   __shared__ int hist[2048];
-  __shared__ int s_digit, s_need, s_cnt_gt, s_cnt_eq, s_fin;
+  __shared__ int s_digit, s_need, s_cnt_gt, s_fin;
+  __shared__ int s_weq[32];                             // per-warp counts of elements equal to the threshold
   const int b = blockIdx.x;
   const TopkSeg S = P.seg[blockIdx.y];
   const float* v = S.vals + (long long)b * S.row_stride;
@@ -135,18 +136,32 @@ topk_segments_kernel(const TopkParams P) {
     T = prefix;
     need = want;
   }
-  if (tid == 0) { s_cnt_gt = 0; s_cnt_eq = 0; s_fin = 0; }
+  if (tid == 0) { s_cnt_gt = 0; s_fin = 0; }
   for (int i = tid; i < k2; i += blockDim.x) sel[i] = 0ull;       // padding sorts last
   __syncthreads();
   int fin = 0;
   const uint32_t ninf = fkey(-INFINITY);
   if (k < n) {
+    // elements above T land in any order (the sort below orders them by (key, index)); of the elements EQUAL to T the
+    // `need` lowest indices are kept — counted in index order (block-wide prefix over the tile), never in atomic
+    // arrival order, so the selected set is the same on every run
     const int base_eq = k - need;
-    for (int i = tid; i < n; i += blockDim.x) {
-      const uint32_t u = fkey(v[i]);
+    const int lane = tid & 31, wid = tid >> 5, nw = (blockDim.x + 31) >> 5;
+    int eq_before = 0;                                        // tied elements in earlier tiles
+    for (int i0 = 0; i0 < n; i0 += blockDim.x) {
+      const int i = i0 + tid;
+      const uint32_t u = i < n ? fkey(v[i]) : 0u;
+      const bool eq = i < n && u == T;
+      const unsigned bal = __ballot_sync(0xffffffffu, eq);
+      if (lane == 0) s_weq[wid] = __popc(bal);
+      __syncthreads();
+      int before = eq_before, tile = 0;
+      for (int w = 0; w < nw; ++w) { const int c = s_weq[w]; tile += c; if (w < wid) before += c; }
+      __syncthreads();                                        // s_weq is rewritten by the next tile
+      eq_before += tile;
       int pos = -1;
-      if (u > T) pos = atomicAdd(&s_cnt_gt, 1);
-      else if (u == T) { const int e = atomicAdd(&s_cnt_eq, 1); if (e < need) pos = base_eq + e; }
+      if (i < n && u > T) pos = atomicAdd(&s_cnt_gt, 1);
+      else if (eq) { const int e = before + __popc(bal & ((1u << lane) - 1u)); if (e < need) pos = base_eq + e; }
       if (pos >= 0) { sel[pos] = ((unsigned long long)u << 32) | (uint32_t)(~(uint32_t)i); fin += u > ninf; }
     }
   } else {

@@ -2,7 +2,7 @@
 
 Same registry names / config keys / state_dict names / call signatures as
 cubercnn/modeling/{meta_arch,backbone,proposal_generator,roi_heads} (SURVEY.md section 8b), with the
-arithmetic running on libc3d.so (sm_100a kernels) — see DESIGN.md for the boundary.
+arithmetic running on libc3d.so (sm_90a kernels) — see DESIGN.md for the boundary.
 """
 from .config import CfgNode, get_cfg, get_cfg_defaults, load_cfg  # noqa: F401
 from .registry import (BACKBONE_REGISTRY, META_ARCH_REGISTRY, PROPOSAL_GENERATOR_REGISTRY,  # noqa: F401

@@ -1,4 +1,4 @@
-"""DLA-34 / ResNet-34 bottom-up + FPN on the tcgen05 convolution kernels (NHWC bf16).
+"""DLA-34 / ResNet-34 bottom-up + FPN on the wgmma convolution kernels (NHWC bf16).
 
 Mirrors the module tree, parameter names and initialisation order of
 cubercnn/modeling/backbone/dla.py:40-68,156-321,417-507 and resnet.py:12-96 (+ detectron2 FPN), so a

@@ -124,8 +124,8 @@ class RCNN3D(nn.Module):
         """RPN anchor labelling + sampling depends on the GT only: run its ~60 small launches on a side stream while
         the backbone occupies the main one (fork/join; also valid inside a CUDA-graph capture).  Every tensor it
         produces stays referenced until after the join, and the side stream allocates nothing outside this region."""
-        if not os.environ.get("C3D_SIDE_STREAM"):      # opt-in: measured 0.4 ms SLOWER per step on B200 (the small
-            return None                                # launches contend with the persistent conv CTAs), profiles/
+        if not os.environ.get("C3D_SIDE_STREAM"):      # opt-in: the small launches contend with the persistent conv
+            return None                                # CTAs
         pg = self.proposal_generator
         Hp, Wp = int(x.shape[1]), int(x.shape[2])
         shapes = []

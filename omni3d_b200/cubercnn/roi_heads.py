@@ -28,7 +28,7 @@ def assign_levels(boxes, min_level=2, max_level=6):
 
 
 def fc(x, lin, relu=False, chw=None, out_fp32=False):
-    """[relu](x W^T + b) on the tcgen05 GEMM (c3d_linear_*).  chw = (C, P*P): W is the reference's weight over a
+    """[relu](x W^T + b) on the wgmma GEMM (c3d_linear_*).  chw = (C, P*P): W is the reference's weight over a
     (C,P,P)-flattened RoI while x is the (P,P,C)-flattened NHWC RoI the ROIAlign kernel emits (features re-ordered
     when the weight is packed to bf16; the weight gradient is written back in the master's order)."""
     return LinearAct.apply(x, lin.weight, lin.bias, relu, out_fp32, chw)
@@ -356,7 +356,7 @@ class ROIHeads3D(nn.Module):
         return cx, cy, dims, pose, raw["z"] * v2r
 
     def cube_losses_fused(self, raw, boxes, classes, valid, gt3, gtR, Kb, v2r):
-        """same quantities as cube_losses(), computed by the fused sm_100a kernel (c3d_cube_loss_fwd/bwd)."""
+        """same quantities as cube_losses(), computed by the fused sm_90a kernel (c3d_cube_loss_fwd/bwd)."""
         from ..nnfunc import CubeLossRows
         w = self.w
         n = boxes.shape[0]

@@ -3,7 +3,7 @@ cubercnn/modeling/proposal_generator/rpn.py:19-354 over detectron2's RPN / Stand
 DefaultAnchorGenerator / find_top_rpn_proposals (SURVEY.md A.3).
 
 All images of the batch are processed together (no per-image Python loop, no .item()/.tolist()):
-  head      3x3 conv + ReLU and the two 1x1 predictors fused into one 16-channel fp32 conv (tcgen05)
+  head      3x3 conv + ReLU and the two 1x1 predictors fused into one 16-channel fp32 conv (wgmma)
   labels    (B,G,A) IoU -> matcher [0.05] with low-quality matches, best-anchor override, ignore regions
   sampling  IoU-weighted sampling without replacement as batched Gumbel top-k on the device
   proposals decode, per-level top-k, clip, c3d_nms_batched (coordinate-trick offsets), top post_nms_topk

@@ -3,7 +3,7 @@
 Mirror of cubercnn/data/dataset_mapper.py:17-155 (DatasetMapper3D.__call__, transform_instance_annotations,
 annotations_to_instances) with the reference's train-time augmentations (detectron2 defaults selected by
 configs/Base.yaml:10-13 + config.py:147: T.ResizeShortestEdge(MIN_SIZE_TRAIN, MAX_SIZE_TRAIN, "choice") and
-T.RandomFlip(horizontal)) re-designed for the B200: the decoded uint8 image goes to the GPU ONCE, as it is; resize
+T.RandomFlip(horizontal)) re-designed for the GPU: the decoded uint8 image goes to the GPU ONCE, as it is; resize
 (Pillow-exact 8-bit bilinear, what detectron2's ResizeTransform calls), flip and the HWC->CHW transposition run there
 (c3d_resize_bilinear_u8) and hand the model the same uint8 (3,H,W) tensor the reference's mapper emits — no CPU resample,
 no deepcopy, no per-image pickle through worker queues.  The few annotation numbers are transformed on the host in float64

@@ -1,4 +1,4 @@
-"""torch.autograd.Function wrappers that put the hand-written sm_100a kernels on the autograd tape.
+"""torch.autograd.Function wrappers that put the hand-written sm_90a kernels on the autograd tape.
 
 Activations are NHWC bf16 tensors (N,H,W,C); parameters stay fp32 masters in the reference's layouts
 (conv weight OIHW, so checkpoints / optimizers see the reference's tensors) and are re-packed to the
@@ -128,8 +128,7 @@ _MERGE_MAX_O = int(os.environ.get("C3D_DGRAD_MERGE_MAX_O", "256"))
 def _merge_phases(I, O):
     """stride-2 3x3 data gradient as ONE 2x2 convolution of dy with 4*I output channels — (row parity, column parity, ci), the
     conv epilogue places the two row halves one dx row apart (c3d.h y_split_*) — instead of four phase convs: 1.78x the
-    FLOPs (7 of the 16 taps are zero) but one pass over dy, one launch, full-width tiles.  Measured (batch 32, B200):
-    16->32 @640: 0.591 -> 0.253 ms, 32->64 @320: 0.312 -> 0.111, 64->128 @160: 0.107 -> 0.070, 128->256 @80: 0.075 -> 0.060."""
+    FLOPs (7 of the 16 taps are zero) but one pass over dy, one launch, full-width tiles."""
     return O <= _MERGE_MAX_O and (2 * I) % 16 == 0 and O % 16 == 0
 
 
@@ -238,7 +237,7 @@ def _grad_slot(p):
 # ---- gradient chaining -------------------------------------------------------------------------------------------------
 # A tensor with several consumers (DLA: block input -> conv1 + residual; tree1 output -> tree2 + Root; Tree input ->
 # pool + strided conv; FPN top-down map -> output conv + the next lateral's addend ...) makes autograd run one add pass
-# per extra consumer over the whole gradient (~1.3 ms / step of strided bf16 adds at batch 32, profiles/r02_summary.md).
+# per extra consumer over the whole gradient.
 # `fork(t, n)` hands every consumer its own alias of t; the aliases share a _GradSink.  The first consumer to produce
 # its gradient parks the buffer in the sink and returns it; every later consumer ADDS INTO that buffer inside the kernel
 # that produces its contribution (conv epilogue add_mode 3, c3d_bn_bwd's accumulating dres, c3d_maxpool2_bwd_acc) and
@@ -428,7 +427,7 @@ def _packed_linear(w, chw):
 
 
 class LinearAct(torch.autograd.Function):
-    """y = [relu](x W^T + b) on the tcgen05 GEMM (c3d_linear_fwd / _dgrad / _wgrad) — the FC layers of
+    """y = [relu](x W^T + b) on the wgmma GEMM (c3d_linear_fwd / _dgrad / _wgrad) — the FC layers of
     FastRCNNConvFCHead / FastRCNNOutputLayers / CubeHead (Base.yaml:67-70, cube_head.py:63-73,108-144).
     x (rows, K) bf16; W fp32 master (N, K) in the reference's layout; chw = (C, PP) when the master's input features are
     ordered (c, p) while x is the NHWC-flattened RoI (p, c)."""

@@ -1,5 +1,5 @@
 """Sync-free train-step harness with the semantics of tools/train_net.py:117-316 (do_train) and
-cubercnn/solver/build.py:6-69 (build_optimizer), re-designed for one-process-per-B200 data parallelism:
+cubercnn/solver/build.py:6-69 (build_optimizer), re-designed for one-process-per-GPU data parallelism:
 
 * parameters live as views into ONE flat fp32 arena (decay | no-decay | unused regions), gradients and
   momentum in matching arenas: one memset zeroes grads, one NCCL all-reduce averages them over NVLink, one
@@ -124,7 +124,7 @@ class FlatSGDTrainer:
         with torch.no_grad():
             for p, off, n in zip(order, offs, sizes):
                 if p.dim() == 4 and channels_last_weights:
-                    # conv weights are STORED (Cout,KH,KW,Cin) — the layout the tcgen05 kernels consume and the
+                    # conv weights are STORED (Cout,KH,KW,Cin) — the layout the wgmma kernels consume and the
                     # weight-gradient kernel produces — and exposed to torch as (Cout,Cin,KH,KW) strided views
                     # (= torch.channels_last); checkpoints and optimizer semantics are unchanged
                     O, I, KH, KW = p.shape

@@ -1,4 +1,4 @@
-"""GPU unit tests of the sm_100a helper kernels against plain PyTorch fp32 references of the same op
+"""GPU unit tests of the sm_90a helper kernels against plain PyTorch fp32 references of the same op
 (tolerances: bf16 storage => 2^-8 relative on outputs; fp32 accumulations 1e-5)."""
 import pytest
 import torch
@@ -350,8 +350,8 @@ def test_fused_proposal_decode_matches_torch_formulation():
                                                 (1, 80, 80, 192, 128, 1, 1), (2, 9, 11, 64, 64, 3, 1)])
 @pytest.mark.parametrize("mode", ["stats", "relu_add", "up2", "fp32"])
 def test_conv_swapped_kernel_epilogue_modes(N, H, W, Cin, Cout, k, s, mode):
-    """Layers with 64 / 128 output channels run the swapped kernel (Cout is the MMA's M, a 256-pixel tile its N; the
-    accumulator is transposed): every epilogue mode on ragged maps (partial tiles in both directions) vs fp32 torch."""
+    """Layers with 64 / 128 output channels (formerly a separate Cout-as-M kernel, now the general persistent kernel):
+    every epilogue mode on ragged maps (partial tiles in both directions) vs fp32 torch."""
     from omni3d_b200 import conv as K
     torch.backends.cudnn.allow_tf32 = False
     p = k // 2
@@ -390,3 +390,35 @@ def test_conv_swapped_kernel_epilogue_modes(N, H, W, Cin, Cout, k, s, mode):
         y = K.conv2d_fwd(x, w, b, stride=s, pad=p, out_fp32=True)
         assert y.dtype == torch.float32
         assert (y - (ref.permute(0, 2, 3, 1) + b)).abs().max().item() <= 2e-3 * ref.abs().max().item() + 1e-4
+
+
+def test_reductions_are_run_to_run_deterministic():
+    """the same inputs give bit-identical results on every call: split-K / per-CTA weight-gradient partials are summed in
+    a fixed order, ROIAlign backward accumulates order-independently, and the top-k keeps the lowest indices of the
+    values tied at its threshold (not the first to arrive)"""
+    from omni3d_b200 import conv as K
+    from omni3d_b200 import kernels as Kx
+    # weight gradients: one many-split GEMM layer and one thin-channel (halo) layer
+    for (N, H, W, Cin, Cout) in [(8, 64, 64, 64, 64), (4, 128, 128, 16, 16)]:
+        x = _r(N, H, W, Cin, seed=1).bfloat16()
+        dy = _r(N, H, W, Cout, seed=2).bfloat16()
+        a = K.conv2d_wgrad(x, dy, 3, 3, 1, 1)
+        b = K.conv2d_wgrad(x, dy, 3, 3, 1, 1)
+        assert torch.equal(a, b), (Cin, Cout)
+    # ROIAlign backward: many overlapping RoIs on one map
+    feats = [_r(2, 64, 64, 64, seed=3).bfloat16()]
+    g = torch.Generator(device="cuda").manual_seed(4)
+    xy = torch.rand(400, 2, device="cuda", generator=g) * 40
+    wh = torch.rand(400, 2, device="cuda", generator=g) * 40 + 8
+    rois = torch.cat([(torch.arange(400, device="cuda") % 2).float()[:, None], torch.zeros(400, 1, device="cuda"),
+                      xy, xy + wh], 1).contiguous()
+    dout = _r(400, 7, 7, 64, seed=5).bfloat16()
+    ga = Kx.roi_align_bwd(feats, [1.0], rois, dout)
+    gb = Kx.roi_align_bwd(feats, [1.0], rois, dout)
+    assert torch.equal(ga[0], gb[0])
+    # top-k with a run of ties at the threshold: the lowest tied indices are kept
+    v = torch.zeros(1, 5000, device="cuda")
+    v[0, 4000:] = 1.0                                    # 1000 values above the tie
+    vals, idx = Kx.topk_segments([(v, 1500)])
+    kept = idx[0, 1000:].long().sort().values
+    assert torch.equal(kept, torch.arange(500, device="cuda"))

@@ -125,7 +125,7 @@ def test_train_losses_with_injected_sampling(pair):
 
 def test_train_losses_and_grads_frozen_bn(pair):
     """Full model, BatchNorm frozen (MODEL.USE_BN False semantics): losses AND parameter gradients of the
-    CUDA path (tcgen05 dgrad/wgrad, BN/ROIAlign backward kernels) against the fp32 oracle."""
+    CUDA path (wgmma dgrad/wgrad, BN/ROIAlign backward kernels) against the fp32 oracle."""
     prod, orc = pair
     from oracle_capture import run_oracle_train, to_injection
     items = synth.make_batch(2, H, W, num_gt=4, seed=2)
@@ -152,8 +152,8 @@ def test_train_losses_and_grads_frozen_bn(pair):
     errs = sorted((_rel(got_g[n].float().cpu(), g), n) for n, g in ref_g.items() if g.norm() > 1e-7)
     med = errs[len(errs) // 2][0]
     p95 = errs[int(0.95 * len(errs))][0]
-    # bf16 activations/gradients through ~35 conv layers + ReLU-mask flips: measured 0.09 median / 0.22 p95 on
-    # B200 (the per-kernel backward tests in test_kernels_gpu.py hold 4e-2); bound it at 0.12 / 0.30
+    # bf16 activations/gradients through ~35 conv layers + ReLU-mask flips (the per-kernel backward tests in
+    # test_kernels_gpu.py hold 4e-2); bound it at 0.12 / 0.30
     assert med < 0.12 and p95 < 0.30, (med, p95, errs[-5:])
 
 

@@ -26,18 +26,23 @@ def test_oracle_matches_reference_run(name):
     sd = model.state_dict()
     assert set(sd) == set(g["init_sum"]), "state_dict key names differ from the reference"
     assert sum(p.numel() for p in model.parameters()) == g["n_params"]
-    for k, v in sd.items():   # same-seed init is bit-identical
-        assert float(v.double().sum()) == g["init_sum"][k] and float(v.double().abs().sum()) == g["init_abs"][k], k
+    for k, v in sd.items():   # same-seed init is bit-identical; only the float64 reduction order of the checksum may
+        # differ between CPUs (vector width), by far less than one changed float32 element would move it
+        assert float(v.double().sum()) == pytest.approx(g["init_sum"][k], rel=1e-13, abs=1e-15), k
+        assert float(v.double().abs().sum()) == pytest.approx(g["init_abs"][k], rel=1e-13, abs=1e-15), k
     model.train()
     torch.manual_seed(123)
     with EventStorage(0) as st:
         losses = model(model_io.to_d2_inputs(synth.make_batch(2, H, W, num_gt=4, seed=1)))
         sum(losses.values()).backward()
         scalars = st.latest()
+    # the fixture was recorded on one CPU; another vector width rounds the fp32 reductions differently in the last bits
     assert list(losses) == list(g["losses"])
     for k in losses:
-        assert torch.equal(losses[k].detach(), g["losses"][k]), k
-    assert scalars == g["scalars"]
+        assert torch.allclose(losses[k].detach(), g["losses"][k], rtol=1e-5, atol=1e-7), k
+    assert set(scalars) == set(g["scalars"])
+    for k, v in scalars.items():
+        assert v == pytest.approx(g["scalars"][k], rel=1e-5, abs=1e-7), k
     assert sorted(n for n, p in model.named_parameters() if p.grad is None) == g["no_grad"]
     for n, p in model.named_parameters():
         if p.grad is not None:
@@ -50,17 +55,21 @@ def test_oracle_matches_reference_run(name):
         f = r["instances"].get_fields()
         assert set(f) == set(d)
         for k, v in f.items():
-            assert torch.equal(v.tensor if hasattr(v, "tensor") else v, d[k]), k
+            v = v.tensor if hasattr(v, "tensor") else v
+            if v.is_floating_point():
+                assert v.shape == d[k].shape and torch.allclose(v, d[k], rtol=1e-4, atol=1e-5), (k, float((v - d[k]).abs().max()))
+            else:
+                assert torch.equal(v, d[k]), k
 
 
 @pytest.mark.parametrize("src", ["repo", "reference"])
 def test_config_surface(src):
-    """the flattened repo configs and (when present) the reference's own YAML chain load to the same values"""
+    """the flattened repo configs and the reference's own YAML chain load to the same values (the reference chain as
+    stored in tests/golden/reference_cfg_DLA34_FPN.yaml: the CfgNode.dump() of its configs/cubercnn_DLA34_FPN.yaml
+    loaded through the oracle's config system)"""
     path = "cubercnn_DLA34_FPN.yaml"
     if src == "reference":
-        path = "/root/reference/configs/cubercnn_DLA34_FPN.yaml"
-        if not os.path.exists(path):
-            pytest.skip("/root/reference not present")
+        path = os.path.join(ROOT, "tests/golden/reference_cfg_DLA34_FPN.yaml")
     cfg = co.load_cfg(path)
     assert cfg.MODEL.META_ARCHITECTURE == "RCNN3D" and cfg.MODEL.ROI_HEADS.NUM_CLASSES == 50
     assert cfg.MODEL.BACKBONE.NAME == "build_dla_from_vision_fpn_backbone"

@@ -1,5 +1,5 @@
 """Round-2 parity tests (VERDICT r1 'what's weak' 1-5): the convolution kernels at the BASELINE shapes that produce the
-headline number (multi-tile persistent CTAs, TMEM double-buffer reuse, full split-K, halo-ring wrap), ResNet34-FPN against
+headline number (multi-tile persistent CTAs, persistent tile loop, full split-K, halo-ring wrap), ResNet34-FPN against
 the oracle, a 640x640 model step, the 3x3/s2 max pool, and the packed-weight cache across CUDA-graph replays."""
 import os
 
@@ -23,7 +23,7 @@ def _rel(a, b):
 
 # name, N, H, W, Cin, Cout, k, stride, pad  — BASELINE configs[1] layer shapes (batch 32 @ 640^2)
 REAL_SHAPES = [
-    ("fpn_out_256@160", 32, 160, 160, 256, 256, 3, 1, 1),      # top kernel: persistent BN=256, 6400 m-tiles / 148 CTAs
+    ("fpn_out_256@160", 32, 160, 160, 256, 256, 3, 1, 1),      # top kernel: persistent BN=256, 6400 m-tiles / 132 CTAs
     ("level0_16@640", 32, 640, 640, 16, 16, 3, 1, 1),          # rolling-halo kernel, ring cycles through 640 rows
     ("l3_128@80", 32, 80, 80, 128, 128, 3, 1, 1),
     ("l2_s2_64to128@160", 32, 160, 160, 64, 128, 3, 2, 1),     # stride-2 entry conv (phase-decomposed data gradient)
@@ -31,13 +31,13 @@ REAL_SHAPES = [
     ("l5_512@20", 32, 20, 20, 512, 512, 3, 1, 1),
     ("fpn_lat_64to256@160", 32, 160, 160, 64, 256, 1, 1, 0),
     ("level1_16to32_s2@640", 32, 640, 640, 16, 32, 3, 2, 1),   # data gradient = ONE merged 2x2 conv of dy (split channel placement)
-    ("l2_entry_32to64_s2@320", 32, 320, 320, 32, 64, 3, 2, 1),  # merged data gradient on the swapped kernel (4*32 = 128 channels)
+    ("l2_entry_32to64_s2@320", 32, 320, 320, 32, 64, 3, 2, 1),  # merged data gradient, 4*32 = 128 channels
 ]
 
 
 @pytest.mark.parametrize("name,N,H,W,Cin,Cout,k,s,p", REAL_SHAPES, ids=[r[0] for r in REAL_SHAPES])
 def test_conv_real_shapes_vs_torch_fp32(name, N, H, W, Cin, Cout, k, s, p):
-    """fwd / dgrad / wgrad of the tcgen05 kernels at the batch-32 640x640 shapes vs F.conv2d in fp32 (TF32 off) on the
+    """fwd / dgrad / wgrad of the wgmma kernels at the batch-32 640x640 shapes vs F.conv2d in fp32 (TF32 off) on the
     same bf16-rounded operands.  Outputs are bf16 => 2^-8 relative; the fp32 weight gradient agrees to accumulation order."""
     from omni3d_b200.nnfunc import ConvBias
     torch.backends.cudnn.allow_tf32 = False
@@ -267,7 +267,7 @@ def test_trainer_state_dict_roundtrip():
         FlatSGDTrainer(pc.load_cfg("cubercnn_DLA34_FPN.yaml", ["MODEL.WEIGHTS_PRETRAIN", "none", "SOLVER.NESTEROV", True]), model2)
 
 
-# ---- FC layers on the tcgen05 GEMM (VERDICT r1 next#4; SURVEY 8a-9 / 8a-10) ------------------------------------------
+# ---- FC layers on the wgmma GEMM (VERDICT r1 next#4; SURVEY 8a-9 / 8a-10) ------------------------------------------
 @pytest.mark.parametrize("rows,C,PP,N,relu,out_fp32", [(384, 64, 4, 256, True, False), (1000, 1024, 1, 256, False, True),
                                                        (4096, 1024, 1, 768, False, True), (16384, 256, 49, 1024, True, False),
                                                        (200, 128, 1, 64, True, False)])

@@ -1,4 +1,4 @@
-"""GPU bring-up probe for the tcgen05 conv kernels: each case runs in its own process under a
+"""GPU bring-up probe for the wgmma conv kernels: each case runs in its own process under a
 timeout (a protocol bug traps or times out without taking the other cases down)."""
 import json
 import os

@@ -1,4 +1,4 @@
-"""Per-shape timing of the tcgen05 conv kernels on the layer shapes of DLA34_FPN @ 640^2, batch 32
+"""Per-shape timing of the wgmma conv kernels on the layer shapes of DLA34_FPN @ 640^2, batch 32
 (SURVEY.md section 8a-2 census): CUDA-event ms and algorithmic TFLOP/s for forward, data gradient and weight
 gradient, with the multiplicity of every shape in one train step, so the table sums to the conv time of a step.
 Also the target of the ncu --set full captures under profiles/ (ONLY=<substring> KIND=fwd|dgrad|wgrad)."""
@@ -48,7 +48,7 @@ N = int(os.environ.get("BATCH", "32"))
 ITERS = int(os.environ.get("ITERS", "5"))
 only = os.environ.get("ONLY")
 kind = os.environ.get("KIND", "fwd,dgrad,wgrad").split(",")
-flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")     # > 126 MB L2
+flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")     # > 50 MB L2 (H100)
 
 
 def timeit(fn):

@@ -1,5 +1,5 @@
 """FC-layer GEMMs of the box / cube heads (configs/Base.yaml:67-70, cube_head.py:63-73): c3d_linear_fwd/_dgrad/_wgrad
-(tcgen05, our kernels) next to the cuBLAS kernels torch picks for the same bf16 GEMMs (the library bar to match)."""
+(wgmma, our kernels) next to the cuBLAS kernels torch picks for the same bf16 GEMMs (the library bar to match)."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
