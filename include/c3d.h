@@ -135,11 +135,14 @@ int32_t c3d_pack_conv_weight(const float* w, int32_t Cout, int32_t Cin, int32_t 
 
 /* every conv weight of a model in one launch: descs_dev = device array of n c3d_pack_desc (forward pack, rotated /
  * transposed data-gradient pack and, for 3x3 stride-2 layers, the four phase sub-kernels of the phase-decomposed data
- * gradient: (Cin, KH', KW', Cout) with parity 0 -> tap [1], parity 1 -> taps [2, 0]); `start` = prefix sum of elements */
+ * gradient: (Cin, KH', KW', Cout) with parity 0 -> tap [1], parity 1 -> taps [2, 0]); `start` = prefix sum of elements.
+ * merged_phases != 0: phase[(a,b) = 2*a+b] are the four row blocks [(2*a+b)*Cin, +Cin) of ONE (4*Cin, 2, 2, Cout) weight
+ * (the merged stride-2 data gradient, see y_split_* of c3d_conv_desc): every phase is stored as 2x2 and the taps it does
+ * not use are left untouched (the caller zeroes them once). */
 typedef struct {
   const float* src; void* fwd; void* dgrad; void* phase[4];
   int64_t start;
-  int32_t Cout, Cin, KH, KW, src_is_ohwi, pad_;
+  int32_t Cout, Cin, KH, KW, src_is_ohwi, merged_phases;
 } c3d_pack_desc;
 int32_t c3d_pack_conv_weights_batched(const void* descs_dev, int32_t n, int64_t total_elems, void* stream);
 

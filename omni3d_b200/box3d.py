@@ -10,11 +10,10 @@ Inputs may be CUDA tensors (used in place) or CPU tensors / arrays (copied to th
 returned on the CPU like the reference, which runs this op on the CPU at
 omni3d_evaluation.py:1404-1412).
 """
-import ctypes
-
 import torch
 
 from . import _lib
+from ._lib import ptr, stream
 
 _ws_cache = {}
 
@@ -45,10 +44,6 @@ def _device_of(*ts):
     return torch.device("cuda", torch.cuda.current_device())
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 def _is_cuda(x):
     return isinstance(x, torch.Tensor) and x.is_cuda
 
@@ -66,9 +61,8 @@ def iou_box3d(boxes1, boxes2, with_counts=False):
         nf = torch.empty((N, M), dtype=torch.int32, device=dev) if with_counts else None
         if N * M > 0:
             ws = _workspace(L.c3d_iou_box3d_workspace_bytes(N, M), dev)
-            st = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check(L.c3d_iou_box3d(_ptr(b1), N, _ptr(b2), M, _ptr(vol), _ptr(iou), _ptr(nf), _ptr(ws),
-                                       ws.numel(), ctypes.c_void_p(st)), launches=4)
+            _lib.check(L.c3d_iou_box3d(ptr(b1), N, ptr(b2), M, ptr(vol), ptr(iou), ptr(nf), ptr(ws),
+                                       ws.numel(), stream(dev)), launches=4)
     out = (vol, iou, nf) if with_counts else (vol, iou)
     return tuple(o.cpu() for o in out) if ret_cpu else out
 
@@ -88,9 +82,8 @@ def iou_box3d_paired(boxes1, boxes2, with_counts=False):
         nf = torch.empty(n, dtype=torch.int32, device=dev) if with_counts else None
         if n > 0:
             ws = _workspace(L.c3d_iou_box3d_workspace_bytes(n, 0), dev)
-            st = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check(L.c3d_iou_box3d_paired(_ptr(b1), _ptr(b2), n, _ptr(vol), _ptr(iou), _ptr(nf), _ptr(ws),
-                                              ws.numel(), ctypes.c_void_p(st)), launches=3)
+            _lib.check(L.c3d_iou_box3d_paired(ptr(b1), ptr(b2), n, ptr(vol), ptr(iou), ptr(nf), ptr(ws),
+                                              ws.numel(), stream(dev)), launches=3)
     out = (vol, iou, nf) if with_counts else (vol, iou)
     return tuple(o.cpu() for o in out) if ret_cpu else out
 
@@ -108,9 +101,8 @@ def box3d_overlap(boxes_dt, boxes_gt, eps_coplanar: float = 1e-4, eps_nonzero: f
         nbad = torch.zeros(2, dtype=torch.int32, device=dev)
         if N > 0:
             ws = _workspace(L.c3d_iou_box3d_workspace_bytes(N, max(M, 1)), dev)
-            st = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check(L.c3d_box3d_overlap(_ptr(b1), N, _ptr(b2), M, eps_coplanar, eps_nonzero, _ptr(iou),
-                                           _ptr(nbad), _ptr(ws), ws.numel(), ctypes.c_void_p(st)), launches=5)
+            _lib.check(L.c3d_box3d_overlap(ptr(b1), N, ptr(b2), M, eps_coplanar, eps_nonzero, ptr(iou),
+                                           ptr(nbad), ptr(ws), ws.numel(), stream(dev)), launches=5)
         bad = nbad.tolist()   # the reference's .any() checks (:158,162) are host syncs too
     if bad[0]:
         print('Warning: skipping {:d} non-coplanar boxes at eval.'.format(int(bad[0])))

@@ -8,64 +8,7 @@ import ctypes
 import torch
 
 from . import _lib
-
-
-class ConvDesc(ctypes.Structure):
-    _fields_ = [("N", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32), ("Cin", ctypes.c_int32),
-                ("Cout", ctypes.c_int32), ("KH", ctypes.c_int32), ("KW", ctypes.c_int32),
-                ("stride", ctypes.c_int32), ("pad", ctypes.c_int32), ("relu", ctypes.c_int32),
-                ("out_fp32", ctypes.c_int32), ("add_mode", ctypes.c_int32),
-                ("x_pix_stride", ctypes.c_int64), ("y_pix_stride", ctypes.c_int64),
-                ("add_pix_stride", ctypes.c_int64), ("y_img_stride", ctypes.c_int64), ("y_h_stride", ctypes.c_int64),
-                ("y_w_stride", ctypes.c_int64), ("y_offset", ctypes.c_int64), ("out_h", ctypes.c_int32),
-                ("out_w", ctypes.c_int32), ("x_img_stride", ctypes.c_int64), ("y_split_c", ctypes.c_int32),
-                ("pad_", ctypes.c_int32), ("y_split_off", ctypes.c_int64)]
-
-
-_bound = False
-
-
-def _bind():
-    global _bound
-    L = _lib.lib()
-    if not _bound:
-        vp, i32 = ctypes.c_void_p, ctypes.c_int32
-        P = ctypes.POINTER(ConvDesc)
-        L.c3d_conv2d_tiles.restype = i32
-        L.c3d_conv2d_tiles.argtypes = [P, ctypes.POINTER(i32), ctypes.POINTER(i32), ctypes.POINTER(i32)]
-        L.c3d_conv2d_fwd.restype = i32
-        L.c3d_conv2d_fwd.argtypes = [P, vp, vp, vp, vp, vp, vp, vp]
-        L.c3d_conv2d_wgrad.restype = i32
-        L.c3d_conv2d_wgrad.argtypes = [P, vp, vp, vp, vp]
-        L.c3d_conv2d_wgrad_ex.restype = i32
-        L.c3d_conv2d_wgrad_ex.argtypes = [P, vp, vp, vp, i32, vp]
-        L.c3d_pack_conv_weight.restype = i32
-        L.c3d_pack_conv_weight.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp]
-        i64 = ctypes.c_int64
-        L.c3d_pack_linear_weight.restype = i32
-        L.c3d_pack_linear_weight.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]
-        L.c3d_linear_fwd.restype = i32
-        L.c3d_linear_fwd.argtypes = [vp, vp, vp, vp, i64, i32, i32, i32, i32, vp]
-        L.c3d_linear_dgrad.restype = i32
-        L.c3d_linear_dgrad.argtypes = [vp, vp, vp, i64, i32, i32, vp]
-        L.c3d_linear_wgrad.restype = i32
-        L.c3d_linear_wgrad.argtypes = [vp, vp, vp, i64, i32, i32, i32, i32, i32, vp]
-        L.c3d_linear_fwd_blocks.restype = i32
-        L.c3d_linear_fwd_blocks.argtypes = [vp, vp, vp, vp, i32, i32, i64, i32, i32, i32, i32, vp]
-        L.c3d_linear_dgrad_blocks.restype = i32
-        L.c3d_linear_dgrad_blocks.argtypes = [vp, vp, vp, i32, i32, i64, i32, i32, i32, vp]
-        L.c3d_linear_wgrad_blocks.restype = i32
-        L.c3d_linear_wgrad_blocks.argtypes = [vp, vp, vp, i32, i32, i64, i32, i32, i32, i32, i32, vp]
-        _bound = True
-    return L
-
-
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+from ._lib import ConvDesc, ptr, stream
 
 
 def out_hw(H, W, KH, KW, stride, pad):
@@ -76,11 +19,12 @@ def make_desc(x, w, stride=1, pad=0, relu=False, out_fp32=False, add_mode=0):
     N, H, W, Cin = x.shape
     Cout, KH, KW, Cin2 = w.shape
     assert Cin == Cin2, (x.shape, w.shape)
-    return ConvDesc(N, H, W, Cin, Cout, KH, KW, stride, pad, int(relu), int(out_fp32), add_mode, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)
+    return ConvDesc(N=N, H=H, W=W, Cin=Cin, Cout=Cout, KH=KH, KW=KW, stride=stride, pad=pad, relu=int(relu),
+                    out_fp32=int(out_fp32), add_mode=add_mode)
 
 
 def num_tiles(desc):
-    L = _bind()
+    L = _lib.lib()
     t, th, tw = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
     _lib.check(L.c3d_conv2d_tiles(ctypes.byref(desc), ctypes.byref(t), ctypes.byref(th), ctypes.byref(tw)))
     return t.value, th.value, tw.value
@@ -91,7 +35,7 @@ def conv2d_fwd(x, w, bias=None, stride=1, pad=0, relu=False, addend=None, up2=Fa
     """x (N,H,W,Cin) bf16, w (Cout,KH,KW,Cin) bf16 -> y (N,Ho,Wo,Cout) bf16|fp32 [, stats (tiles,2,Cout)].
     out: write into this buffer (dense, or a channel slice of a wider NHWC tensor); accumulate: out += conv (add_mode 3,
     fp32 add in the epilogue) instead of out = conv."""
-    L = _bind()
+    L = _lib.lib()
     assert x.is_cuda and x.dtype == torch.bfloat16 and x.is_contiguous()
     assert w.dtype == torch.bfloat16 and w.is_contiguous()
     add_mode = 0 if addend is None else (2 if up2 else 1)
@@ -125,14 +69,14 @@ def conv2d_fwd(x, w, bias=None, stride=1, pad=0, relu=False, addend=None, up2=Fa
         assert bias.dtype == torch.float32 and bias.is_contiguous()
     if addend is not None:
         assert addend.dtype == torch.bfloat16 and addend.is_contiguous()
-    _lib.check(L.c3d_conv2d_fwd(ctypes.byref(d), _ptr(x), _ptr(w), _ptr(bias), _ptr(addend), _ptr(out), _ptr(stats),
-                                _stream()))
+    _lib.check(L.c3d_conv2d_fwd(ctypes.byref(d), ptr(x), ptr(w), ptr(bias), ptr(addend), ptr(out), ptr(stats),
+                                stream()))
     return (out, stats) if want_stats else out
 
 
 def pack_conv_weight(w, want_fwd=True, want_dgrad=True):
     """fp32 (Cout,Cin,KH,KW) -> bf16 (Cout,KH,KW,Cin) and bf16 (Cin,KH,KW,Cout) rotated, in ONE launch."""
-    L = _bind()
+    L = _lib.lib()
     Cout, Cin, KH, KW = w.shape
     w = w.detach()
     ohwi = (not w.is_contiguous()) and w.permute(0, 2, 3, 1).is_contiguous()     # channels_last master storage
@@ -140,20 +84,20 @@ def pack_conv_weight(w, want_fwd=True, want_dgrad=True):
         w = w.contiguous()
     f = torch.empty((Cout, KH, KW, Cin), device=w.device, dtype=torch.bfloat16) if want_fwd else None
     g = torch.empty((Cin, KH, KW, Cout), device=w.device, dtype=torch.bfloat16) if want_dgrad else None
-    _lib.check(L.c3d_pack_conv_weight(_ptr(w), Cout, Cin, KH, KW, int(ohwi), _ptr(f), _ptr(g), _stream()))
+    _lib.check(L.c3d_pack_conv_weight(ptr(w), Cout, Cin, KH, KW, int(ohwi), ptr(f), ptr(g), stream()))
     return f, g
 
 
 def conv2d_wgrad(x, dy, KH, KW, stride=1, pad=0, dw=None, oihw=False):
     """dW (Cout,KH,KW,Cin) [or (Cout,Cin,KH,KW) when oihw] fp32 (+)= wgrad(x (N,H,W,Cin) bf16, dy bf16)."""
-    L = _bind()
+    L = _lib.lib()
     N, H, W, Cin = x.shape
     Cout = dy.shape[3]
     assert x.dtype == torch.bfloat16 and dy.dtype == torch.bfloat16 and x.is_contiguous() and dy.is_contiguous()
     if dw is None:
         dw = torch.zeros((Cout, Cin, KH, KW) if oihw else (Cout, KH, KW, Cin), device=x.device, dtype=torch.float32)
-    d = ConvDesc(N, H, W, Cin, Cout, KH, KW, stride, pad, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)
-    _lib.check(L.c3d_conv2d_wgrad_ex(ctypes.byref(d), _ptr(x), _ptr(dy), _ptr(dw), int(oihw), _stream()))
+    d = ConvDesc(N=N, H=H, W=W, Cin=Cin, Cout=Cout, KH=KH, KW=KW, stride=stride, pad=pad)
+    _lib.check(L.c3d_conv2d_wgrad_ex(ctypes.byref(d), ptr(x), ptr(dy), ptr(dw), int(oihw), stream()))
     return dw
 
 
@@ -161,81 +105,81 @@ def conv2d_wgrad(x, dy, KH, KW, stride=1, pad=0, dw=None, oihw=False):
 def pack_linear_weight(w, chw=None, want_t=True):
     """fp32 master (N, K) -> bf16 (N, K') [+ bf16 (K', N)].  chw = (C, PP): the master's input features are ordered
     (c, p) (nn.Linear over an NCHW-flattened RoI) and are re-ordered to (p, c) (NHWC-flattened RoI)."""
-    L = _bind()
+    L = _lib.lib()
     N, Kdim = w.shape
     w = w.detach().contiguous()
     C, PP = chw if chw is not None else (Kdim, 1)
     f = torch.empty((N, Kdim), device=w.device, dtype=torch.bfloat16)
     t = torch.empty((Kdim, N), device=w.device, dtype=torch.bfloat16) if want_t else None
-    _lib.check(L.c3d_pack_linear_weight(_ptr(w), N, Kdim, C, PP, _ptr(f), _ptr(t), _stream()), launches=2 if want_t else 1)
+    _lib.check(L.c3d_pack_linear_weight(ptr(w), N, Kdim, C, PP, ptr(f), ptr(t), stream()), launches=2 if want_t else 1)
     return f, t
 
 
 def linear_fwd(x, w, bias=None, relu=False, out_fp32=False):
     """x (rows, K) bf16, w (N, K) bf16, bias (N,) fp32 -> [relu](x w^T + bias) (rows, N) bf16 | fp32."""
-    L = _bind()
+    L = _lib.lib()
     rows, Kdim = x.shape
     N = w.shape[0]
     assert x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.is_contiguous() and w.is_contiguous()
     assert w.shape[1] == Kdim and (bias is None or (bias.dtype == torch.float32 and bias.is_contiguous()))
     y = torch.empty((rows, N), device=x.device, dtype=torch.float32 if out_fp32 else torch.bfloat16)
-    _lib.check(L.c3d_linear_fwd(_ptr(x), _ptr(w), _ptr(bias), _ptr(y), rows, Kdim, N, int(relu), int(out_fp32), _stream()))
+    _lib.check(L.c3d_linear_fwd(ptr(x), ptr(w), ptr(bias), ptr(y), rows, Kdim, N, int(relu), int(out_fp32), stream()))
     return y
 
 
 def linear_dgrad(dy, wt):
     """dy (rows, N) bf16, wt (K, N) bf16 (the transposed weight) -> dx (rows, K) bf16."""
-    L = _bind()
+    L = _lib.lib()
     rows, N = dy.shape
     Kdim = wt.shape[0]
     assert dy.dtype == torch.bfloat16 and wt.dtype == torch.bfloat16 and dy.is_contiguous() and wt.is_contiguous()
     dx = torch.empty((rows, Kdim), device=dy.device, dtype=torch.bfloat16)
-    _lib.check(L.c3d_linear_dgrad(_ptr(dy), _ptr(wt), _ptr(dx), rows, N, Kdim, _stream()))
+    _lib.check(L.c3d_linear_dgrad(ptr(dy), ptr(wt), ptr(dx), rows, N, Kdim, stream()))
     return dx
 
 
 def linear_wgrad(x, dy, dw=None, chw=None, master_chw=True):
     """dw (N, K) fp32 (+)= dy^T x.  chw = (C, PP) + master_chw: address dw in the master's (c, p) feature order."""
-    L = _bind()
+    L = _lib.lib()
     rows, Kdim = x.shape
     N = dy.shape[1]
     assert x.dtype == torch.bfloat16 and dy.dtype == torch.bfloat16 and x.is_contiguous() and dy.is_contiguous()
     if dw is None:
         dw = torch.zeros((N, Kdim), device=x.device, dtype=torch.float32)
     C, PP = chw if chw is not None else (Kdim, 1)
-    _lib.check(L.c3d_linear_wgrad(_ptr(x), _ptr(dy), _ptr(dw), rows, Kdim, N, C, PP, int(bool(master_chw and chw is not None)),
-                                  _stream()))
+    _lib.check(L.c3d_linear_wgrad(ptr(x), ptr(dy), ptr(dw), rows, Kdim, N, C, PP, int(bool(master_chw and chw is not None)),
+                                  stream()))
     return dw
 
 
 def linear_fwd_blocks(x, nseg, seg_rows, seg_stride, w, bias=None, relu=False, out_fp32=False):
     """rows [b*seg_stride, b*seg_stride + seg_rows) of x (.., K), b < nseg, read in place -> dense (nseg*seg_rows, N)."""
-    L = _bind()
+    L = _lib.lib()
     Kdim, N = x.shape[1], w.shape[0]
     assert x.dtype == torch.bfloat16 and x.is_contiguous() and w.is_contiguous() and (nseg - 1) * seg_stride + seg_rows <= x.shape[0]
     y = torch.empty((nseg * seg_rows, N), device=x.device, dtype=torch.float32 if out_fp32 else torch.bfloat16)
-    _lib.check(L.c3d_linear_fwd_blocks(_ptr(x), _ptr(w), _ptr(bias), _ptr(y), nseg, seg_rows, seg_stride, Kdim, N, int(relu),
-                                       int(out_fp32), _stream()))
+    _lib.check(L.c3d_linear_fwd_blocks(ptr(x), ptr(w), ptr(bias), ptr(y), nseg, seg_rows, seg_stride, Kdim, N, int(relu),
+                                       int(out_fp32), stream()))
     return y
 
 
 def linear_dgrad_blocks(dy, wt, dx, nseg, seg_rows, seg_stride, accumulate=True):
     """dx rows [b*seg_stride, +seg_rows) (+)= dy (nseg*seg_rows, N) . W, in place inside the larger dx (.., K)."""
-    L = _bind()
+    L = _lib.lib()
     N, Kdim = dy.shape[1], wt.shape[0]
     assert dy.dtype == torch.bfloat16 and dy.is_contiguous() and dx.dtype == torch.bfloat16 and dx.is_contiguous()
     assert dx.shape[1] == Kdim and (nseg - 1) * seg_stride + seg_rows <= dx.shape[0] and dy.shape[0] == nseg * seg_rows
-    _lib.check(L.c3d_linear_dgrad_blocks(_ptr(dy), _ptr(wt), _ptr(dx), nseg, seg_rows, seg_stride, N, Kdim, int(accumulate), _stream()))
+    _lib.check(L.c3d_linear_dgrad_blocks(ptr(dy), ptr(wt), ptr(dx), nseg, seg_rows, seg_stride, N, Kdim, int(accumulate), stream()))
     return dx
 
 
 def linear_wgrad_blocks(x, dy, nseg, seg_rows, seg_stride, dw=None, chw=None, master_chw=True):
-    L = _bind()
+    L = _lib.lib()
     Kdim, N = x.shape[1], dy.shape[1]
     assert x.dtype == torch.bfloat16 and dy.dtype == torch.bfloat16 and x.is_contiguous() and dy.is_contiguous()
     if dw is None:
         dw = torch.zeros((N, Kdim), device=x.device, dtype=torch.float32)
     C, PP = chw if chw is not None else (Kdim, 1)
-    _lib.check(L.c3d_linear_wgrad_blocks(_ptr(x), _ptr(dy), _ptr(dw), nseg, seg_rows, seg_stride, Kdim, N, C, PP,
-                                         int(bool(master_chw and chw is not None)), _stream()))
+    _lib.check(L.c3d_linear_wgrad_blocks(ptr(x), ptr(dy), ptr(dw), nseg, seg_rows, seg_stride, Kdim, N, C, PP,
+                                         int(bool(master_chw and chw is not None)), stream()))
     return dw

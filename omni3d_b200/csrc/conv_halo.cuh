@@ -385,13 +385,8 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
-static bool halo_enabled() {
-  static const bool on = getenv("C3D_CONV_NO_HALO") == nullptr;
-  return on;
-}
 // pure function of the descriptor (c3d_conv2d_tiles must agree with c3d_conv2d_fwd)
 static bool halo_fwd_eligible(const c3d_conv_desc* d) {
-  if (!halo_enabled()) return false;
   if (d->stride != 1 || d->KH != d->KW || !(d->KH & 1) || 2 * d->pad != d->KH - 1) return false;
   if (d->out_h > 0 || d->out_w > 0 || d->add_mode != 0) return false;
   if (!(d->Cin == 8 || d->Cin == 16 || d->Cin == 32)) return false;
@@ -401,7 +396,6 @@ static bool halo_fwd_eligible(const c3d_conv_desc* d) {
   return true;
 }
 static bool halo_wgrad_eligible(const c3d_conv_desc* d) {
-  if (!halo_enabled()) return false;
   if (d->stride != 1 || d->KH != d->KW || !(d->KH & 1) || 2 * d->pad != d->KH - 1) return false;
   if (!(d->Cin == 8 || d->Cin == 16 || d->Cin == 32)) return false;
   if (!(d->Cout == 16 || d->Cout == 32)) return false;
@@ -409,13 +403,10 @@ static bool halo_wgrad_eligible(const c3d_conv_desc* d) {
   if (d->W < 128 && d->Cin != 8) return false;
   return (d->KH == 7 && d->Cin == 8) || (d->KH == 3 && d->Cin >= 16);     // the compiled instances
 }
-// ring depth: the TMA rows are only 2-4 KB, so hiding ~1.5 us of L2/HBM latency at ~40 B/ns per SM needs tens of rows in
-// flight; C3D_HALO_PREFETCH overrides the number of rows beyond the filter window
+// ring depth: the TMA rows are only 2-4 KB, so hiding ~1.5 us of L2/HBM latency at ~40 B/ns per SM needs tens of rows in flight
 static int halo_ring_rows(int window, int slot_bytes, int budget) {
-  static const char* env = getenv("C3D_HALO_PREFETCH");
   int pf = budget / slot_bytes - window;
   if (pf > 48) pf = 48;
-  if (env) pf = atoi(env);
   if (pf < 2) pf = 2;
   return window + pf;
 }

@@ -300,25 +300,24 @@ struct WgradKParams {
                                              // spatial shift; KH/KW/Cin only drive the epilogue's master-layout index
 };
 
-// PIX = pixels (GEMM K) per pipeline stage: 128 px x 2 stages or 64 px x 4 stages (same 192 KB).  The larger box fits
-// feature maps whose rows do not tile into 64-pixel boxes (20x20 -> 4x20).
-template <int STAGES, int PIX, int NCOLS = 256>
+// two pipeline stages of kPix pixels (GEMM K) x up to kCols GEMM columns per CTA (192 KB)
 struct WgradSmem {
-  static constexpr int kABytes = PIX * 128 * 2;            // up to two [PIX px][64 ch] chunks (or narrower)
-  static constexpr int kBBytes = PIX * NCOLS * 2;          // NCOLS columns x PIX pixels
-  static constexpr int kStageBytes = kABytes + kBBytes;    // 96 KB (PIX 128) / 48 KB (PIX 64)
-  static constexpr int kBarOffset = STAGES * kStageBytes;
+  static constexpr int kStages = 2, kPix = 128, kCols = 256;
+  static constexpr int kABytes = kPix * 128 * 2;           // up to two [kPix px][64 ch] chunks (or narrower)
+  static constexpr int kBBytes = kPix * kCols * 2;         // kCols columns x kPix pixels
+  static constexpr int kStageBytes = kABytes + kBBytes;    // 96 KB
+  static constexpr int kBarOffset = kStages * kStageBytes;
   static constexpr int kTotal = kBarOffset + 256 + 1024;
 };
 
 // main loop + epilogue of one consumer warpgroup with an NB-column accumulator (NB >= the CTA's columns rounded up to
 // 64; the extra columns read stale shared memory and are never stored)
-template <int NB, int STAGES, int PIX, int NCOLS>
+template <int NB>
 __device__ __forceinline__ void wgrad_consume(const WgradKParams& P, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                               const int t_begin, const int t_end, const int warp, const int lane,
                                               const int co0, const int box0, const int ncols, const uint32_t a_box_bytes,
                                               const uint32_t b_box_bytes) {
-  using S = WgradSmem<STAGES, PIX, NCOLS>;
+  using S = WgradSmem;
   const int wg = warp >> 2;
   const bool active = co0 + wg * 64 < P.Cout;        // this warpgroup's 64 output channels exist
   float acc[NB / 2];
@@ -346,7 +345,7 @@ __device__ __forceinline__ void wgrad_consume(const WgradKParams& P, uint8_t* sm
     }
     if (prev >= 0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty_bar[prev]); }
     prev = stage;
-    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    if (++stage == S::kStages) { stage = 0; phase ^= 1; }
   }
   ptx::wgmma_wait<0>();
   ptx::fence_regs(acc);
@@ -408,34 +407,33 @@ static int32_t with_ordered_partials(int nparts, long long welems, float* dw, cu
   return rc;
 }
 
-template <int STAGES, int PIX, int NCOLS = 256>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
                      const WgradKParams P) {
-  using S = WgradSmem<STAGES, PIX, NCOLS>;
+  using S = WgradSmem;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
-  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* empty_bar = full_bar + S::kStages;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   const int split = blockIdx.x, group = blockIdx.y, co_tile = blockIdx.z;
   const int co0 = co_tile * 128;
   const int box0 = group * P.boxes_per_cta;
   const int nb = min(P.boxes_per_cta, P.total_boxes - box0);       // boxes (taps x ci chunks) of this CTA
-  const int ncols = nb * P.cw;                                     // GEMM N (multiple of 16, <= NCOLS)
+  const int ncols = nb * P.cw;                                     // GEMM N (multiple of 16, <= S::kCols)
   const int t_begin = split * P.tiles_per_split;
   const int t_end = min(P.num_tiles, t_begin + P.tiles_per_split);
   if (t_begin >= t_end) return;
   const int R = P.RH * P.RW;
   int a_chunks = (P.Cout - co0 + P.ca - 1) / P.ca;
   if (a_chunks > P.a_chunks_max) a_chunks = P.a_chunks_max;
-  // distance between channel chunks in shared memory: a full PIX-pixel slot per box, or (5-D boxes) the dense box pitch
-  const uint32_t a_box_bytes = (uint32_t)((P.big ? R : PIX) * P.ca * 2), b_box_bytes = (uint32_t)((P.big ? R : PIX) * P.cw * 2);
+  // distance between channel chunks in shared memory: a full kPix-pixel slot per box, or (5-D boxes) the dense box pitch
+  const uint32_t a_box_bytes = (uint32_t)((P.big ? R : S::kPix) * P.ca * 2), b_box_bytes = (uint32_t)((P.big ? R : S::kPix) * P.cw * 2);
 
   if (warp == kConsumerWarps && lane == 0) {
     ptx::prefetch_tensormap(&tmap_dy); ptx::prefetch_tensormap(&tmap_x);
-    for (int s = 0; s < STAGES; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kConsumerWarps); }
+    for (int s = 0; s < S::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kConsumerWarps); }
     ptx::fence_barrier_init();
   }
   __syncthreads();
@@ -477,23 +475,24 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
                                wo0 * P.stride + kw - P.pad, ho0 * P.stride + kh - P.pad, img);
           }
         }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if (++stage == S::kStages) { stage = 0; phase ^= 1; }
       }
     }
   } else {
-    if (NCOLS > 192 && ncols > 192)
-      wgrad_consume<(NCOLS > 192 ? 256 : 64), STAGES, PIX, NCOLS>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
-    else if (NCOLS > 128 && ncols > 128)
-      wgrad_consume<(NCOLS > 128 ? 192 : 64), STAGES, PIX, NCOLS>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
+    if (ncols > 192)
+      wgrad_consume<256>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
+    else if (ncols > 128)
+      wgrad_consume<192>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
     else if (ncols > 64)
-      wgrad_consume<128, STAGES, PIX, NCOLS>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
+      wgrad_consume<128>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
     else
-      wgrad_consume<64, STAGES, PIX, NCOLS>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
+      wgrad_consume<64>(P, smem, full_bar, empty_bar, t_begin, t_end, warp, lane, co0, box0, ncols, a_box_bytes, b_box_bytes);
   }
 }
 
-// pixel box for wgrad: RH*RW must be a multiple of 16 (wgmma K) and <= max_pix; returns the covered fraction
-static double pick_tile_k(int Ho, int Wo, int stride, int* RH, int* RW, int max_pix = 128) {
+// pixel box for wgrad: RH*RW must be a multiple of 16 (wgmma K) and <= WgradSmem::kPix
+static void pick_tile_k(int Ho, int Wo, int stride, int* RH, int* RW) {
+  constexpr int max_pix = WgradSmem::kPix;
   double best = -1; int bth = 1, btw = 16;
   for (int tw = 1; tw <= max_pix; ++tw) {
     if (tw * stride > 256) break;
@@ -506,7 +505,6 @@ static double pick_tile_k(int Ho, int Wo, int stride, int* RH, int* RW, int max_
     }
   }
   *RH = bth; *RW = btw;
-  return best;
 }
 
 }  // namespace c3d
@@ -656,22 +654,14 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
       return set_error(C3D_EINVAL, "linear wgrad: bad feature factorisation %d x %d != %d", lin_c, lin_pp, Cin);
     P.Cin = lin_c; P.KH = lin_pp; P.KW = 1;      // epilogue index space: (tap = p, ci = c); the loader ignores kh / kw
   }
-  // 64-pixel stages (4-deep pipeline) unless the map tiles clearly better into 128-pixel boxes
-  int rh64, rw64;
-  const double eff128 = pick_tile_k(Ho, Wo, d->stride, &P.RH, &P.RW, 128);
-  const double eff64 = pick_tile_k(Ho, Wo, d->stride, &rh64, &rw64, 64);
-  // opt-in experiments: the 4 x 64-pixel pipeline, and 128 instead of 256 GEMM columns per CTA
-  static const bool want64 = getenv("C3D_WGRAD_PIX64") != nullptr;
-  static const bool n128 = getenv("C3D_WGRAD_N128") != nullptr;
-  const bool pix64 = want64 && eff64 >= 0.93 * eff128;
-  if (pix64) { P.RH = rh64; P.RW = rw64; }
+  pick_tile_k(Ho, Wo, d->stride, &P.RH, &P.RW);
   P.tiles_h = (Ho + P.RH - 1) / P.RH; P.tiles_w = (Wo + P.RW - 1) / P.RW;
   P.num_tiles = d->N * P.tiles_h * P.tiles_w;
   const int taps = P.KH * P.KW;
   const int Cin_e = P.Cin;                       // channels per tap in the epilogue's index space
   P.cw = (Cin_e % 64 == 0) ? 64 : (Cin_e % 32 == 0 ? 32 : 16);
   P.nci = Cin_e / P.cw;
-  P.boxes_per_cta = (n128 ? 128 : 256) / P.cw;
+  P.boxes_per_cta = WgradSmem::kCols / P.cw;
   P.total_boxes = taps * P.nci;
   P.ca = (Cout % 64 == 0) ? 64 : (Cout % 32 == 0 ? 32 : 16);
   P.a_chunks_max = 128 / P.ca;    // chunks beyond Cout are not loaded (those D rows are never stored)
@@ -695,9 +685,8 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   CUtensorMap mdy, mx;
   // 5-D maps (channel-chunk axis OUTSIDE the pixel axes): one box = [chunks][RH][RW][64 ch], the MN-major operand layout
   // with LBO = RH*RW*128 B — a third of the TMA instructions per stage (the loop is bound by boxes issued, not bytes)
-  static const bool no_big = getenv("C3D_WGRAD_NO_BIGBOX") != nullptr;
   P.big = 0; P.mc = 1;
-  if (!no_big) {
+  {
     const int nchunks_x = P.lin ? P.total_boxes : P.nci;
     int mc = P.boxes_per_cta;
     while (mc > 1 && nchunks_x % mc != 0) mc >>= 1;
@@ -750,23 +739,15 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<2, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         WgradSmem<2, 128>::kTotal);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<4, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               WgradSmem<4, 64>::kTotal);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<3, 128, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               WgradSmem<3, 128, 128>::kTotal);
+    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         WgradSmem::kTotal);
     if (e != cudaSuccess) return set_error(C3D_ECUDA, "wgrad smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
   return with_ordered_partials(splits, welems, dw, st, [&](float* part) -> int32_t {
     WgradKParams Q = P;
     Q.part = part;
-    if (n128 && !pix64) conv_wgrad_tc_kernel<3, 128, 128><<<grid, kGemmThreads, WgradSmem<3, 128, 128>::kTotal, st>>>(mdy, mx, Q);
-    else if (pix64) conv_wgrad_tc_kernel<4, 64><<<grid, kGemmThreads, WgradSmem<4, 64>::kTotal, st>>>(mdy, mx, Q);
-    else conv_wgrad_tc_kernel<2, 128><<<grid, kGemmThreads, WgradSmem<2, 128>::kTotal, st>>>(mdy, mx, Q);
+    conv_wgrad_tc_kernel<<<grid, kGemmThreads, WgradSmem::kTotal, st>>>(mdy, mx, Q);
     return check_launch("conv_wgrad_tc_kernel");
   });
 }

@@ -589,19 +589,14 @@ __global__ void pack_conv_weight_kernel(const float* __restrict__ w, int Cout, i
 // stride-2 phase sub-kernels): every source element writes its forward-pack entry, its rotated / transposed data-gradient
 // entry and — for 3x3 stride-2 layers — its entry in the phase sub-kernel it belongs to (nnfunc._phase_packs:
 // parity 0 uses tap [1], parity 1 taps [2, 0]).
-struct PackDesc {
-  const float* src; bf16* fwd; bf16* dgrad; bf16* phase[4];
-  long long start;                 // first global element index of this tensor
-  int Cout, Cin, KH, KW, ohwi, pad_;
-};
-__global__ void pack_conv_weights_batched_kernel(const PackDesc* __restrict__ descs, int n, long long total) {
+__global__ void pack_conv_weights_batched_kernel(const c3d_pack_desc* __restrict__ descs, int n, long long total) {
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     int lo = 0, hi = n;
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (descs[mid].start <= e) lo = mid; else hi = mid; }
-    const PackDesc D = descs[lo];
+    const c3d_pack_desc D = descs[lo];
     const long long i = e - D.start;
     int kw, kh, ci, co;
-    if (D.ohwi) {
+    if (D.src_is_ohwi) {
       ci = (int)(i % D.Cin); long long t = i / D.Cin;
       kw = (int)(t % D.KW); t /= D.KW;
       kh = (int)(t % D.KH); co = (int)(t / D.KH);
@@ -611,15 +606,14 @@ __global__ void pack_conv_weights_batched_kernel(const PackDesc* __restrict__ de
       ci = (int)(t % D.Cin); co = (int)(t / D.Cin);
     }
     const bf16 v = __float2bfloat16(D.src[i]);
-    if (D.fwd) D.fwd[(((long long)co * D.KH + kh) * D.KW + kw) * D.Cin + ci] = v;
-    if (D.dgrad) D.dgrad[(((long long)ci * D.KH + (D.KH - 1 - kh)) * D.KW + (D.KW - 1 - kw)) * D.Cout + co] = v;
+    if (D.fwd) static_cast<bf16*>(D.fwd)[(((long long)co * D.KH + kh) * D.KW + kw) * D.Cin + ci] = v;
+    if (D.dgrad) static_cast<bf16*>(D.dgrad)[(((long long)ci * D.KH + (D.KH - 1 - kh)) * D.KW + (D.KW - 1 - kw)) * D.Cout + co] = v;
     if (D.phase[0]) {               // 3x3 only: parity a = (kh != 1), position inside the phase: kh 1 -> 0 | kh 2 -> 0, kh 0 -> 1
       const int a = kh != 1, b = kw != 1;
       const int ph = a ? (kh == 2 ? 0 : 1) : 0, pw = b ? (kw == 2 ? 0 : 1) : 0;
-      // pad_ != 0: "merged" layout — the four phases are row blocks [(a,b)*Cin, +Cin) of ONE (4*Cin, 2, 2, Cout) weight (a 2x2
-      // convolution of dy with 4*Cin output channels, include/c3d.h y_split_*); taps a phase does not use stay zero
-      const int KHp = (a || D.pad_) ? 2 : 1, KWp = (b || D.pad_) ? 2 : 1;
-      D.phase[a * 2 + b][(((long long)ci * KHp + ph) * KWp + pw) * D.Cout + co] = v;
+      // merged_phases: every phase is a 2x2 row block of one (4*Cin, 2, 2, Cout) weight (include/c3d.h c3d_pack_desc)
+      const int KHp = (a || D.merged_phases) ? 2 : 1, KWp = (b || D.merged_phases) ? 2 : 1;
+      static_cast<bf16*>(D.phase[a * 2 + b])[(((long long)ci * KHp + ph) * KWp + pw) * D.Cout + co] = v;
     }
   }
 }
@@ -838,9 +832,8 @@ extern "C" int32_t c3d_preprocess_image_u8(const uint8_t* img, int32_t H, int32_
 }
 extern "C" int32_t c3d_pack_conv_weights_batched(const void* descs_dev, int32_t n, int64_t total_elems, void* stream) {
   C3D_REQ(descs_dev && n > 0 && total_elems > 0, "pack_conv_weights_batched: bad args");
-  static_assert(sizeof(PackDesc) == 88, "c3d_pack_desc layout");
-  pack_conv_weights_batched_kernel<<<grid_for(total_elems, 256), 256, 0, (cudaStream_t)stream>>>((const PackDesc*)descs_dev, n,
-                                                                                                 total_elems);
+  pack_conv_weights_batched_kernel<<<grid_for(total_elems, 256), 256, 0, (cudaStream_t)stream>>>(
+      static_cast<const c3d_pack_desc*>(descs_dev), n, total_elems);
   return check_launch("pack_conv_weights_batched");
 }
 extern "C" int32_t c3d_preprocess_batch(const void* const* imgs_host, const int32_t* H_host, const int32_t* W_host, int32_t N,

@@ -275,8 +275,7 @@ static int32_t nms_impl(const float* boxes, const int32_t* nvalid, const float* 
   // rows whose diagonal tile is skipped (beyond nvalid) are never read; no memset needed because the scan
   // only reads words >= i/64 of rows i < nvalid, all of which kernel 1 writes when col0 < nvalid.
   if (cats && !maxc) return set_error(C3D_EINVAL, "nms: cats given without maxc");
-  static const bool single_list = getenv("C3D_NMS_SINGLE_LIST") != nullptr;
-  if (cats && ncat > 0 && ncat <= kMaxCat && !single_list) {
+  if (cats && ncat > 0 && ncat <= kMaxCat) {
     // workspace: [mask][perm int32 B*n][cat_off int32 B*(kMaxCat+1)][keepflag u8 B*n]
     uint8_t* base = (uint8_t*)workspace + (((size_t)B * n * words * 8 + 255) & ~(size_t)255);
     int* perm = (int*)base;

@@ -7,7 +7,6 @@ nn.Conv2d / nn.BatchNorm2d modules below are PARAMETER HOLDERS (their forward is
 convolution / BatchNorm / pooling runs through omni3d_b200.nnfunc on libc3d.so).
 """
 import math
-import os
 
 import torch
 import torch.nn.functional as F
@@ -140,7 +139,7 @@ class DLA34(nn.Module):
     out_channels = {"p2": 64, "p3": 128, "p4": 256, "p5": 512, "p6": 512}
     strides = {"p2": 4, "p3": 8, "p4": 16, "p5": 32, "p6": 64}
     # the 7x7 stride-1 stem runs on the rolling-halo kernel, which takes the image as NHWC8 (3 real channels)
-    stem_cpad = 16 if os.environ.get("C3D_CONV_NO_HALO") else 8
+    stem_cpad = 8
 
     def __init__(self):
         super().__init__()

@@ -13,7 +13,6 @@ exactly like the reference and collated into the padded device tensors RCNN3D.st
     shortest_edge_shape(h, w, size, max_size)               -> (new_h, new_w)   (ResizeShortestEdge.get_output_shape)
     DeviceMapper3D(cfg, is_train)(record[, size, flip])     -> {"image", "height", "width", "K", "gt"}
 """
-import ctypes
 import math
 
 import numpy as np
@@ -22,19 +21,7 @@ import torch
 from . import _lib
 
 PRECISION_BITS = 32 - 8 - 2
-_bound = False
 _coef_cache = {}
-
-
-def _bind():
-    global _bound
-    L = _lib.lib()
-    if not _bound:
-        vp, i32 = ctypes.c_void_p, ctypes.c_int32
-        L.c3d_resize_bilinear_u8.restype = i32
-        L.c3d_resize_bilinear_u8.argtypes = [vp, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]
-        _bound = True
-    return L
 
 
 def pil_bilinear_coeffs(in_size, out_size):
@@ -90,7 +77,7 @@ def shortest_edge_shape(h, w, size, max_size):
 def resize_flip_u8(img, new_h, new_w, flip=False):
     """img (H,W,3) uint8 (CUDA tensor, or host tensor / array: copied once) -> (3,new_h,new_w) uint8 CUDA tensor equal to
     np.asarray(Image.fromarray(img).resize((new_w,new_h), BILINEAR))[:, ::-1 if flip].transpose(2,0,1)."""
-    L = _bind()
+    L = _lib.lib()
     if not torch.cuda.is_available():
         raise _lib.C3DError("omni3d_b200.data needs a CUDA device (no CPU fallback)")
     if not isinstance(img, torch.Tensor):
@@ -105,10 +92,9 @@ def resize_flip_u8(img, new_h, new_w, flip=False):
     bv, kv, ksv, first, last = _coeffs_dev(H, new_h, dev)
     tmp = torch.empty((H, new_w, C), dtype=torch.uint8, device=dev)
     out = torch.empty((C, new_h, new_w), dtype=torch.uint8, device=dev)
-    st = torch.cuda.current_stream(dev).cuda_stream
     _lib.check(L.c3d_resize_bilinear_u8(img.data_ptr(), H, W, C, bh.data_ptr(), kh.data_ptr(), ksh, bv.data_ptr(), kv.data_ptr(), ksv,
                                         new_h, new_w, first, last, int(bool(flip)), tmp.data_ptr(), out.data_ptr(),
-                                        ctypes.c_void_p(st)), launches=2)
+                                        _lib.stream(dev)), launches=2)
     return out
 
 

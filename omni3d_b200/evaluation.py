@@ -14,29 +14,11 @@ Semantics kept from the reference: detections sorted by -score with a stable (me
 `[]` when a group has no detections and no ground truths, or when either side is empty (:1414-1415); dt rows that fail the
 planarity / non-zero-volume checks are zeroed and counted in the printed warning (:158-164), once for the whole batch.
 """
-import ctypes
-
 import numpy as np
 import torch
 
 from . import _lib
 from .box3d import _device_of, _workspace
-
-_bound = False
-
-
-def _bind():
-    global _bound
-    L = _lib.lib()
-    if not _bound:
-        vp, i32, i64, f32, sz = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_size_t
-        L.c3d_box3d_overlap_segmented_workspace_bytes.restype = sz
-        L.c3d_box3d_overlap_segmented_workspace_bytes.argtypes = [i64, i64, i64]
-        L.c3d_box3d_overlap_segmented.restype = i32
-        L.c3d_box3d_overlap_segmented.argtypes = [vp, i64, vp, i64, vp, vp, vp, i32, i64, f32, f32, vp, vp, vp, sz, vp]
-        _bound = True
-    return L
-
 
 def _as_boxes(x):
     a = np.asarray(x, dtype=np.float32)
@@ -52,7 +34,7 @@ def box3d_overlap_segmented(dt_groups, gt_groups, eps_coplanar=1e-4, eps_nonzero
     One launch for all groups; equals box3d_overlap(dt_i, gt_i) of every group bit for bit."""
     if len(dt_groups) != len(gt_groups):
         raise ValueError("dt_groups and gt_groups must have the same length")
-    L = _bind()
+    L = _lib.lib()
     G = len(dt_groups)
     dts = [_as_boxes(d.cpu() if isinstance(d, torch.Tensor) else d) for d in dt_groups]
     gts = [_as_boxes(g.cpu() if isinstance(g, torch.Tensor) else g) for g in gt_groups]
@@ -74,10 +56,9 @@ def box3d_overlap_segmented(dt_groups, gt_groups, eps_coplanar=1e-4, eps_nonzero
             iou = torch.empty(max(total, 1), dtype=torch.float32, device=dev)
             nbad = torch.zeros(2, dtype=torch.int32, device=dev)
             ws = _workspace(L.c3d_box3d_overlap_segmented_workspace_bytes(n_dt, max(n_gt, 1), total), dev)
-            st = torch.cuda.current_stream(dev).cuda_stream
             _lib.check(L.c3d_box3d_overlap_segmented(b1.data_ptr(), n_dt, b2.data_ptr(), n_gt, d_off.data_ptr(), g_off.data_ptr(),
                                                      p_off.data_ptr(), G, total, eps_coplanar, eps_nonzero, iou.data_ptr(),
-                                                     nbad.data_ptr(), ws.data_ptr(), ws.numel(), ctypes.c_void_p(st)), launches=5)
+                                                     nbad.data_ptr(), ws.data_ptr(), ws.numel(), _lib.stream(dev)), launches=5)
             out = iou[:total].cpu().numpy()
             bad = nbad.tolist()
     if bad[0]:

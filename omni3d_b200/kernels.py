@@ -5,115 +5,30 @@ import ctypes
 import torch
 
 from . import _lib
+from ._lib import ptr, stream
 
-_bound = False
-vp, i32, i64, f32, f64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double
-
-
-class RoiLevels(ctypes.Structure):
-    _fields_ = [("feat", vp * 5), ("grad", vp * 5), ("H", i32 * 5), ("W", i32 * 5), ("scale", f32 * 5),
-                ("num_levels", i32), ("num_images", i32)]
-
-
-class TopkSeg(ctypes.Structure):
-    _fields_ = [("vals", vp), ("row_stride", i64), ("n", i32), ("k", i32), ("out_col", i32)]
-
-
-class LabelSampleArgs(ctypes.Structure):
-    _fields_ = [("prop_boxes", vp), ("prop_count", vp), ("gt_boxes", vp), ("gt_classes", vp), ("gt_present", vp),
-                ("gt_boxes3D", vp), ("gt_poses", vp), ("B", i32), ("P", i32), ("G", i32), ("K", i32), ("S", i32),
-                ("Fcap", i32), ("append_gt", i32), ("iou_thresh", f32), ("ignore_thresh", f32), ("rng", vp),
-                ("bump_rng", i32), ("matched_idx", vp), ("matched_iou", vp), ("labels", vp), ("s_boxes", vp),
-                ("s_valid", vp), ("s_classes", vp), ("s_gt_boxes", vp), ("s_gt_boxes3D", vp), ("s_gt_poses", vp),
-                ("s_index", vp), ("stats", vp)]
-
-
-def _bind():
-    global _bound
-    L = _lib.lib()
-    if _bound:
-        return L
-    sig = {
-        "c3d_bn_finalize": [vp, i32, i32, f64, f32, f32, vp, vp, vp, vp, vp, vp],
-        "c3d_bn_apply": [vp, vp, vp, vp, vp, vp, i32, vp, i64, i32, i64, i64, vp],
-        "c3d_bn_bwd_blocks": [i64, i32],
-        "c3d_bn_bwd": [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64, vp, vp],
-        "c3d_maxpool2_fwd": [vp, vp, i32, i32, i32, i32, i64, i64, vp],
-        "c3d_maxpool2_bwd": [vp, vp, vp, i32, i32, i32, i32, i64, i64, vp],
-        "c3d_maxpool2_bwd_acc": [vp, vp, vp, i32, i32, i32, i32, i64, i64, i64, vp],
-        "c3d_preprocess_image": [vp, i32, i32, vp, i32, i32, i32, ctypes.POINTER(f32), ctypes.POINTER(f32), vp],
-        "c3d_grad_finite": [vp, i64, vp, vp],
-        "c3d_sgd_momentum": [vp, vp, vp, i64, f32, f32, f32, f32, vp, vp],
-        "c3d_sgd_momentum_dev": [vp, vp, vp, i64, vp, f32, f32, f32, vp, vp],
-        "c3d_roi_align_fwd": [ctypes.POINTER(RoiLevels), vp, i32, i32, i32, i32, vp, vp],
-        "c3d_roi_align_bwd": [ctypes.POINTER(RoiLevels), vp, i32, i32, i32, i32, vp, vp],
-    }
-    sig["c3d_bias_act_bwd"] = [vp, vp, i32, i32, vp, vp, vp, i64, i32, vp, vp]
-    sig["c3d_sumpool2"] = [vp, vp, i32, i32, i32, i32, vp]
-    sig["c3d_cube_loss_fwd"] = [vp, vp, i32, vp, vp]
-    sig["c3d_cube_loss_bwd"] = [vp, vp, vp, i32, vp, vp]
-    sig["c3d_zero_stuff2"] = [vp, vp, i32, i32, i32, i32, i32, i32, vp]
-    sig["c3d_maxpool3s2_fwd"] = [vp, vp, i32, i32, i32, i32, vp]
-    sig["c3d_maxpool3s2_bwd"] = [vp, vp, vp, i32, i32, i32, i32, i64, vp]
-    L.c3d_bn_scratch_bytes.restype = ctypes.c_size_t
-    L.c3d_bn_scratch_bytes.argtypes = [i32]
-    L.c3d_nms_workspace_bytes.restype = ctypes.c_size_t
-    L.c3d_nms_workspace_bytes.argtypes = [i32, i32]
-    sig["c3d_nms_batched"] = [vp, vp, vp, vp, i32, i32, i32, f32, i32, vp, vp, vp, ctypes.c_size_t, vp]
-    sig["c3d_nms_batched_grouped"] = [vp, vp, vp, vp, i32, i32, i32, f32, i32, i32, i32, vp, vp, vp, ctypes.c_size_t, vp]
-    sig["c3d_rpn_loss_fwd"] = [vp, vp, vp, vp, vp, vp, i32, i64, i32, ctypes.POINTER(f32), vp, vp]
-    sig["c3d_rpn_loss_bwd"] = [vp, vp, vp, vp, vp, vp, i32, i64, i32, ctypes.POINTER(f32), vp, vp, vp, vp, vp]
-    sig["c3d_rpn_decode_level"] = [vp, vp, i64, vp, vp, vp, i32, i32, i64, ctypes.POINTER(f32), f32, f32, i32, i32, i32, vp, vp, vp,
-                                   vp, vp, vp]
-    sig["c3d_anchor_match"] = [vp, i64, vp, vp, vp, i32, i32, f32, vp, vp, vp, vp, vp, vp, vp]
-    sig["c3d_preprocess_image_u8"] = [vp, i32, i32, vp, i32, i32, i32, ctypes.POINTER(f32), ctypes.POINTER(f32), vp]
-    sig["c3d_topk_segments"] = [ctypes.POINTER(TopkSeg), i32, i32, i32, vp, vp, vp, vp, vp]
-    sig["c3d_label_sample_proposals"] = [ctypes.POINTER(LabelSampleArgs), vp]
-    sig["c3d_anchor_sample_keys"] = [vp, vp, i32, i64, vp, vp, vp, vp]
-    sig["c3d_box_loss_fwd"] = [vp, i32, vp, vp, vp, vp, i32, i32, ctypes.POINTER(f32), vp, vp]
-    sig["c3d_box_loss_bwd"] = [vp, i32, vp, vp, vp, vp, i32, i32, ctypes.POINTER(f32), vp, vp, vp, vp]
-    sig["c3d_cube_gather"] = [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, vp, vp, vp]
-    sig["c3d_cube_reduce_fwd"] = [vp, vp, i32, vp, vp, vp]
-    sig["c3d_cube_reduce_bwd"] = [vp, vp, i32, vp, vp, vp, vp]
-    sig["c3d_cube_scatter"] = [vp, vp, i32, i32, i32, vp, vp]
-    sig["c3d_preprocess_batch"] = [vp, vp, vp, i32, i32, vp, i32, i32, i32, ctypes.POINTER(f32), ctypes.POINTER(f32), vp]
-    sig["c3d_det_candidates"] = [vp, vp, vp, vp, i32, i32, i32, f32, vp, vp, vp, vp, vp]
-    sig["c3d_anchor_sample_finish"] = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i64, i32, i32, i32, f32, vp, vp, vp]
-    for name, args in sig.items():
-        fn = getattr(L, name)
-        fn.restype = i32
-        fn.argtypes = args
-    _bound = True
-    return L
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _st():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+vp, i32, f32 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_float
 
 
 def bn_finalize(stats, count, eps, momentum, running_mean, running_var):
-    L = _bind()
+    L = _lib.lib()
     rows, _, C = stats.shape
     mean = torch.empty(C, device=stats.device, dtype=torch.float32)
     rstd = torch.empty(C, device=stats.device, dtype=torch.float32)
     scratch = torch.empty(128 * 2 * C + 64, device=stats.device, dtype=torch.float64)
-    _lib.check(L.c3d_bn_finalize(_p(stats), rows, C, float(count), eps, momentum, _p(running_mean), _p(running_var),
-                                 _p(mean), _p(rstd), _p(scratch), _st()), launches=1)
+    _lib.check(L.c3d_bn_finalize(ptr(stats), rows, C, float(count), eps, momentum, ptr(running_mean), ptr(running_var),
+                                 ptr(mean), ptr(rstd), ptr(scratch), stream()), launches=1)
     return mean, rstd
 
 
 def bn_apply(y, mean, rstd, gamma, beta, residual=None, relu=True, out=None):
-    L = _bind()
+    L = _lib.lib()
     C = y.shape[-1]
     P = y.numel() // C
     if out is None:
         out = torch.empty_like(y)
-    _lib.check(L.c3d_bn_apply(_p(y), _p(mean), _p(rstd), _p(gamma), _p(beta), _p(residual), int(relu), _p(out), P, C,
-                              0, 0, _st()))
+    _lib.check(L.c3d_bn_apply(ptr(y), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(residual), int(relu), ptr(out), P, C,
+                              0, 0, stream()))
     return out
 
 
@@ -135,7 +50,7 @@ def bn_bwd(dout, out, y, mean, rstd, gamma, relu, dgamma, dbeta, want_dres, froz
     """-> dy (bf16, like y), dres (bf16 or None); dgamma/dbeta (fp32 [C]) are accumulated in place.  `dout` may be a
     channel slice of a wider NHWC gradient (read in place through its pixel stride).  dres_into: an existing gradient
     buffer of the residual tensor (possibly a channel slice): the masked dout is ADDED into it in place."""
-    L = _bind()
+    L = _lib.lib()
     ds = pixel_stride(dout)
     if ds is None:
         dout, ds = dout.contiguous(), 0
@@ -153,22 +68,22 @@ def bn_bwd(dout, out, y, mean, rstd, gamma, relu, dgamma, dbeta, want_dres, froz
     else:
         dres = torch.empty_like(y) if want_dres else None
     scratch = torch.empty(128 * 2 * C + 64, device=y.device, dtype=torch.float64)
-    _lib.check(L.c3d_bn_bwd(_p(dout), _p(out), _p(y), _p(mean), _p(rstd), _p(gamma), _p(beta), flags, int(frozen), _p(partial), _p(coef),
-                            _p(dgamma), _p(dbeta), _p(dy), _p(dres), P, C, ds, 0, rs, _p(scratch), _st()), launches=3)
+    _lib.check(L.c3d_bn_bwd(ptr(dout), ptr(out), ptr(y), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), flags, int(frozen), ptr(partial), ptr(coef),
+                            ptr(dgamma), ptr(dbeta), ptr(dy), ptr(dres), P, C, ds, 0, rs, ptr(scratch), stream()), launches=3)
     return dy, dres
 
 
 def maxpool2_fwd(x):
-    L = _bind()
+    L = _lib.lib()
     N, H, W, C = x.shape
     y = torch.empty((N, H // 2, W // 2, C), device=x.device, dtype=x.dtype)
-    _lib.check(L.c3d_maxpool2_fwd(_p(x), _p(y), N, H, W, C, 0, 0, _st()))
+    _lib.check(L.c3d_maxpool2_fwd(ptr(x), ptr(y), N, H, W, C, 0, 0, stream()))
     return y
 
 
 def maxpool2_bwd(x, dy, into=None):
     """into: an existing gradient buffer of x (possibly a channel slice) that the routed dy is ADDED to in place."""
-    L = _bind()
+    L = _lib.lib()
     N, H, W, C = x.shape
     ds = pixel_stride(dy)
     if ds is None:
@@ -176,35 +91,35 @@ def maxpool2_bwd(x, dy, into=None):
     if into is not None:
         xs = pixel_stride(into)
         assert xs is not None and into.dtype == torch.bfloat16
-        _lib.check(L.c3d_maxpool2_bwd_acc(_p(x), _p(dy), _p(into), N, H, W, C, 0, ds, xs, _st()))
+        _lib.check(L.c3d_maxpool2_bwd_acc(ptr(x), ptr(dy), ptr(into), N, H, W, C, 0, ds, xs, stream()))
         return into
     dx = torch.empty_like(x)
-    _lib.check(L.c3d_maxpool2_bwd(_p(x), _p(dy), _p(dx), N, H, W, C, 0, ds, _st()))
+    _lib.check(L.c3d_maxpool2_bwd(ptr(x), ptr(dy), ptr(dx), N, H, W, C, 0, ds, stream()))
     return dx
 
 
 def maxpool3s2_fwd(x):
-    L = _bind()
+    L = _lib.lib()
     N, H, W, C = x.shape
     y = torch.empty((N, (H - 1) // 2 + 1, (W - 1) // 2 + 1, C), device=x.device, dtype=x.dtype)
-    _lib.check(L.c3d_maxpool3s2_fwd(_p(x), _p(y), N, H, W, C, _st()))
+    _lib.check(L.c3d_maxpool3s2_fwd(ptr(x), ptr(y), N, H, W, C, stream()))
     return y
 
 
 def maxpool3s2_bwd(x, dy):
-    L = _bind()
+    L = _lib.lib()
     N, H, W, C = x.shape
     ds = pixel_stride(dy)
     if ds is None:
         dy, ds = dy.contiguous(), 0
     dx = torch.empty_like(x)
-    _lib.check(L.c3d_maxpool3s2_bwd(_p(x), _p(dy), _p(dx), N, H, W, C, ds, _st()))
+    _lib.check(L.c3d_maxpool3s2_bwd(ptr(x), ptr(dy), ptr(dx), N, H, W, C, ds, stream()))
     return dx
 
 
 def preprocess_images(images, mean, std, size_divisibility=64, cpad=16):
     """list of (3,H,W) fp32 or uint8 CUDA tensors -> (N,Hp,Wp,cpad) bf16 NHWC batch (normalised, zero padded)."""
-    L = _bind()
+    L = _lib.lib()
     Hm = max(im.shape[1] for im in images)
     Wm = max(im.shape[2] for im in images)
     d = size_divisibility
@@ -220,18 +135,18 @@ def preprocess_images(images, mean, std, size_divisibility=64, cpad=16):
         ptrs = (vp * n)(*[im.data_ptr() for im in images])
         hs = (i32 * n)(*[im.shape[1] for im in images])
         ws = (i32 * n)(*[im.shape[2] for im in images])
-        _lib.check(L.c3d_preprocess_batch(ptrs, hs, ws, n, int(dt == torch.uint8), _p(out), Hp, Wp, cpad, m, s, _st()),
+        _lib.check(L.c3d_preprocess_batch(ptrs, hs, ws, n, int(dt == torch.uint8), ptr(out), Hp, Wp, cpad, m, s, stream()),
                    launches=(n + 63) // 64)
         return out
     for i, im in enumerate(images):
         assert im.dtype in (torch.float32, torch.uint8) and im.is_contiguous() and im.is_cuda
         fn = L.c3d_preprocess_image if im.dtype == torch.float32 else L.c3d_preprocess_image_u8
-        _lib.check(fn(_p(im), im.shape[1], im.shape[2], _p(out[i]), Hp, Wp, cpad, m, s, _st()))
+        _lib.check(fn(ptr(im), im.shape[1], im.shape[2], ptr(out[i]), Hp, Wp, cpad, m, s, stream()))
     return out
 
 
 def _levels(feats, strides, grads=None):
-    lv = RoiLevels()
+    lv = _lib.RoiLevels()
     lv.num_levels = len(feats)
     lv.num_images = feats[0].shape[0]
     for i, f in enumerate(feats):
@@ -244,39 +159,39 @@ def _levels(feats, strides, grads=None):
 
 def roi_align_fwd(feats, strides, rois, pooled=7):
     """feats: list of (N,H,W,C) bf16; rois (R,6) fp32 [batch, level, x1,y1,x2,y2] -> (R,pooled,pooled,C) bf16."""
-    L = _bind()
+    L = _lib.lib()
     C = feats[0].shape[-1]
     R = rois.shape[0]
     out = torch.empty((R, pooled, pooled, C), device=feats[0].device, dtype=torch.bfloat16)
     lv = _levels(feats, strides)
-    _lib.check(L.c3d_roi_align_fwd(ctypes.byref(lv), _p(rois), R, C, pooled, pooled, _p(out), _st()))
+    _lib.check(L.c3d_roi_align_fwd(ctypes.byref(lv), ptr(rois), R, C, pooled, pooled, ptr(out), stream()))
     return out
 
 
 def roi_align_bwd(feats, strides, rois, dout, pooled=7):
     """-> list of fp32 gradient maps shaped like feats."""
-    L = _bind()
+    L = _lib.lib()
     C = feats[0].shape[-1]
     grads = [torch.zeros(f.shape, device=f.device, dtype=torch.float32) for f in feats]
     lv = _levels(feats, strides, grads)
-    _lib.check(L.c3d_roi_align_bwd(ctypes.byref(lv), _p(rois), rois.shape[0], C, pooled, pooled, _p(dout), _st()))
+    _lib.check(L.c3d_roi_align_bwd(ctypes.byref(lv), ptr(rois), rois.shape[0], C, pooled, pooled, ptr(dout), stream()))
     return grads
 
 
 def grad_finite(flat_grad, flag):
-    L = _bind()
-    _lib.check(L.c3d_grad_finite(_p(flat_grad), flat_grad.numel(), _p(flag), _st()))
+    L = _lib.lib()
+    _lib.check(L.c3d_grad_finite(ptr(flat_grad), flat_grad.numel(), ptr(flag), stream()))
 
 
 def sgd_momentum(p, g, mom, lr, momentum, weight_decay, grad_scale=1.0, skip_flag=None):
     """lr: python float, or a 1-element fp32 CUDA tensor (read by the kernel at run time: CUDA-graph friendly)."""
-    L = _bind()
+    L = _lib.lib()
     if torch.is_tensor(lr):
-        _lib.check(L.c3d_sgd_momentum_dev(_p(p), _p(g), _p(mom), p.numel(), _p(lr), momentum, weight_decay, grad_scale,
-                                          _p(skip_flag), _st()))
+        _lib.check(L.c3d_sgd_momentum_dev(ptr(p), ptr(g), ptr(mom), p.numel(), ptr(lr), momentum, weight_decay, grad_scale,
+                                          ptr(skip_flag), stream()))
     else:
-        _lib.check(L.c3d_sgd_momentum(_p(p), _p(g), _p(mom), p.numel(), lr, momentum, weight_decay, grad_scale,
-                                      _p(skip_flag), _st()))
+        _lib.check(L.c3d_sgd_momentum(ptr(p), ptr(g), ptr(mom), p.numel(), lr, momentum, weight_decay, grad_scale,
+                                      ptr(skip_flag), stream()))
 
 
 _nms_ws = {}
@@ -286,7 +201,7 @@ def nms_batched(boxes, nvalid, iou_thresh, max_keep, cats=None, maxc=None, trick
     """boxes (B,n,4) fp32 sorted by score desc, nvalid (B,) int32, cats (B,n) fp32 categories, maxc (B,) fp32
     -> keep_idx (B,max_keep) int32 (-1 padded, score order), keep_cnt (B,) int32.  No host sync.
     ncat > 0: the categories are exactly the integers 0..ncat-1 -> per-category kernels (same result, less work)."""
-    L = _bind()
+    L = _lib.lib()
     B, n, _ = boxes.shape
     boxes = boxes.contiguous()
     need = L.c3d_nms_workspace_bytes(B, n)
@@ -298,19 +213,19 @@ def nms_batched(boxes, nvalid, iou_thresh, max_keep, cats=None, maxc=None, trick
     keep = torch.empty((B, max_keep), dtype=torch.int32, device=boxes.device)
     cnt = torch.empty((B,), dtype=torch.int32, device=boxes.device)
     if ncat > 0 and cats is not None:
-        _lib.check(L.c3d_nms_batched_grouped(_p(boxes), _p(nvalid), _p(cats), _p(maxc), trick_max_numel, B, n, iou_thresh,
-                                             max_keep, ncat, max_per_cat, _p(keep), _p(cnt), _p(ws), ws.numel(), _st()),
+        _lib.check(L.c3d_nms_batched_grouped(ptr(boxes), ptr(nvalid), ptr(cats), ptr(maxc), trick_max_numel, B, n, iou_thresh,
+                                             max_keep, ncat, max_per_cat, ptr(keep), ptr(cnt), ptr(ws), ws.numel(), stream()),
                    launches=4)
         return keep, cnt
-    _lib.check(L.c3d_nms_batched(_p(boxes), _p(nvalid), _p(cats), _p(maxc), trick_max_numel, B, n, iou_thresh,
-                                 max_keep, _p(keep), _p(cnt), _p(ws), ws.numel(), _st()), launches=2)
+    _lib.check(L.c3d_nms_batched(ptr(boxes), ptr(nvalid), ptr(cats), ptr(maxc), trick_max_numel, B, n, iou_thresh,
+                                 max_keep, ptr(keep), ptr(cnt), ptr(ws), ws.numel(), stream()), launches=2)
     return keep, cnt
 
 
 def anchor_match(anchors, gt_boxes, gt_valid, gt_ign, fg_thresh):
     """anchors (A,4), gt_boxes (B,G,4) fp32, gt_valid / gt_ign (B,G) bool -> matched_idx (B,A) int64, matched_iou (B,A),
     labels (B,A) int8 {0,1}, max_ioa (B,A), best_idx (B,G) int32 (A for non-valid GTs)."""
-    L = _bind()
+    L = _lib.lib()
     A = anchors.shape[0]
     B, G, _ = gt_boxes.shape
     dev = anchors.device
@@ -322,8 +237,8 @@ def anchor_match(anchors, gt_boxes, gt_valid, gt_ign, fg_thresh):
     lab = torch.empty((B, A), dtype=torch.int8, device=dev)
     best = torch.empty((B, G), dtype=torch.int32, device=dev)
     ws = torch.empty((B, G), dtype=torch.int32, device=dev)
-    _lib.check(L.c3d_anchor_match(_p(anchors), A, _p(gt_boxes), _p(v8), _p(i8), B, G, float(fg_thresh), _p(idx), _p(iou),
-                                  _p(lab), _p(ioa), _p(best), _p(ws), _st()), launches=3)
+    _lib.check(L.c3d_anchor_match(ptr(anchors), A, ptr(gt_boxes), ptr(v8), ptr(i8), B, G, float(fg_thresh), ptr(idx), ptr(iou),
+                                  ptr(lab), ptr(ioa), ptr(best), ptr(ws), stream()), launches=3)
     return idx, iou, lab, ioa, best
 
 
@@ -331,40 +246,40 @@ def rpn_decode_level(topk_idx, topk_score, deltas, anchors, image_hw, weights, s
                      key, lvl, nvalid, maxc):
     """decode one level's top-k candidates into columns col0.. of boxes (B,Ktot,4) / key / lvl (B,Ktot); nvalid (B,) int32
     and maxc (B,) fp32 accumulate (zero them first)."""
-    L = _bind()
+    L = _lib.lib()
     B, K = topk_idx.shape
     w = (f32 * 4)(*[float(v) for v in weights])
     assert topk_idx.dtype == torch.int64 and topk_idx.stride(1) == 1 and topk_score.stride() == topk_idx.stride()
-    _lib.check(L.c3d_rpn_decode_level(_p(topk_idx), _p(topk_score), topk_idx.stride(0), _p(deltas), _p(anchors), _p(image_hw), B, K,
+    _lib.check(L.c3d_rpn_decode_level(ptr(topk_idx), ptr(topk_score), topk_idx.stride(0), ptr(deltas), ptr(anchors), ptr(image_hw), B, K,
                                       deltas.shape[1], w, float(scale_clamp), float(min_size), int(level), int(col0),
-                                      boxes.shape[1], _p(boxes), _p(key), _p(lvl), _p(nvalid), _p(maxc), _st()))
+                                      boxes.shape[1], ptr(boxes), ptr(key), ptr(lvl), ptr(nvalid), ptr(maxc), stream()))
 
 
 def rpn_loss_fwd(logits, deltas, labels, matched_idx, gt_boxes, anchors, weights):
     """-> acc (6,) fp32: [sum cls, sum loc, #pos, #neg, sum sigmoid over positives, sum sigmoid over the rest]."""
-    L = _bind()
+    L = _lib.lib()
     B, A = logits.shape
     acc = torch.empty(6, dtype=torch.float32, device=logits.device)
     w = (f32 * 4)(*[float(v) for v in weights])
-    _lib.check(L.c3d_rpn_loss_fwd(_p(logits), _p(deltas), _p(labels), _p(matched_idx), _p(gt_boxes), _p(anchors), B, A,
-                                  gt_boxes.shape[1], w, _p(acc), _st()))
+    _lib.check(L.c3d_rpn_loss_fwd(ptr(logits), ptr(deltas), ptr(labels), ptr(matched_idx), ptr(gt_boxes), ptr(anchors), B, A,
+                                  gt_boxes.shape[1], w, ptr(acc), stream()))
     return acc
 
 
 def rpn_loss_bwd(logits, deltas, labels, matched_idx, gt_boxes, anchors, weights, g_cls, g_loc):
-    L = _bind()
+    L = _lib.lib()
     B, A = logits.shape
     dl = torch.empty_like(logits)
     dd = torch.empty_like(deltas)
     w = (f32 * 4)(*[float(v) for v in weights])
-    _lib.check(L.c3d_rpn_loss_bwd(_p(logits), _p(deltas), _p(labels), _p(matched_idx), _p(gt_boxes), _p(anchors), B, A,
-                                  gt_boxes.shape[1], w, _p(g_cls), _p(g_loc), _p(dl), _p(dd), _st()))
+    _lib.check(L.c3d_rpn_loss_bwd(ptr(logits), ptr(deltas), ptr(labels), ptr(matched_idx), ptr(gt_boxes), ptr(anchors), B, A,
+                                  gt_boxes.shape[1], w, ptr(g_cls), ptr(g_loc), ptr(dl), ptr(dd), stream()))
     return dl, dd
 
 
 def bias_act_bwd(dout, out, relu, dbias):
     """dz (bf16) = dout * (out > 0 if relu); dbias (fp32 [C] or None) += sum over pixels."""
-    L = _bind()
+    L = _lib.lib()
     C = dout.shape[-1]
     P = dout.numel() // C
     dout = dout.contiguous()
@@ -376,40 +291,40 @@ def bias_act_bwd(dout, out, relu, dbias):
         return dout
     dz = None if alias else torch.empty(dout.shape, device=dout.device, dtype=torch.bfloat16)
     flags = int(dout.dtype == torch.float32) | (2 if (out is not None and out.dtype == torch.float32) else 0)
-    _lib.check(L.c3d_bias_act_bwd(_p(dout), _p(out), int(relu), flags, _p(dz), _p(partial),
-                                  _p(dbias), P, C, _p(scratch), _st()), launches=2 if dbias is not None else 1)
+    _lib.check(L.c3d_bias_act_bwd(ptr(dout), ptr(out), int(relu), flags, ptr(dz), ptr(partial),
+                                  ptr(dbias), P, C, ptr(scratch), stream()), launches=2 if dbias is not None else 1)
     return dout if alias else dz
 
 
 def sumpool2(x):
-    L = _bind()
+    L = _lib.lib()
     N, H, W, C = x.shape
     y = torch.empty((N, H // 2, W // 2, C), device=x.device, dtype=x.dtype)
-    _lib.check(L.c3d_sumpool2(_p(x), _p(y), N, H, W, C, _st()))
+    _lib.check(L.c3d_sumpool2(ptr(x), ptr(y), N, H, W, C, stream()))
     return y
 
 
 def zero_stuff2(dy, H, W):
-    L = _bind()
+    L = _lib.lib()
     N, Ho, Wo, C = dy.shape
     z = torch.empty((N, H, W, C), device=dy.device, dtype=dy.dtype)
-    _lib.check(L.c3d_zero_stuff2(_p(dy), _p(z), N, Ho, Wo, H, W, C, _st()))
+    _lib.check(L.c3d_zero_stuff2(ptr(dy), ptr(z), N, Ho, Wo, H, W, C, stream()))
     return z
 
 
 def cube_loss_fwd(raw, aux):
-    L = _bind()
+    L = _lib.lib()
     n = raw.shape[0]
     out = torch.empty((n, 10), device=raw.device, dtype=torch.float32)
-    _lib.check(L.c3d_cube_loss_fwd(_p(raw), _p(aux), n, _p(out), _st()))
+    _lib.check(L.c3d_cube_loss_fwd(ptr(raw), ptr(aux), n, ptr(out), stream()))
     return out
 
 
 def cube_loss_bwd(raw, aux, dout):
-    L = _bind()
+    L = _lib.lib()
     n = raw.shape[0]
     draw = torch.empty((n, 13), device=raw.device, dtype=torch.float32)
-    _lib.check(L.c3d_cube_loss_bwd(_p(raw), _p(aux), _p(dout), n, _p(draw), _st()))
+    _lib.check(L.c3d_cube_loss_bwd(ptr(raw), ptr(aux), ptr(dout), n, ptr(draw), stream()))
     return draw
 
 
@@ -438,10 +353,10 @@ def rng_state(device, seed=None):
 def topk_segments(segs, want_idx64=False, want_counts=False):
     """segs: list of (vals (B,n) fp32 [row-strided ok], k).  -> vals (B, sum k) sorted descending inside every segment,
     idx (B, sum k) int32 or int64 (index inside the segment's row) [, counts (B, nseg) of values > -inf]."""
-    L = _bind()
+    L = _lib.lib()
     B = segs[0][0].shape[0]
     dev = segs[0][0].device
-    arr = (TopkSeg * len(segs))()
+    arr = (_lib.TopkSeg * len(segs))()
     col = 0
     keep = []
     for i, (v, k) in enumerate(segs):
@@ -452,8 +367,8 @@ def topk_segments(segs, want_idx64=False, want_counts=False):
     out_v = torch.empty((B, col), dtype=torch.float32, device=dev)
     out_i = torch.empty((B, col), dtype=torch.int64 if want_idx64 else torch.int32, device=dev)
     cnt = torch.empty((B, len(segs)), dtype=torch.int32, device=dev) if want_counts else None
-    _lib.check(L.c3d_topk_segments(arr, len(segs), B, col, _p(out_v), None if want_idx64 else _p(out_i),
-                                   _p(out_i) if want_idx64 else None, _p(cnt), _st()))
+    _lib.check(L.c3d_topk_segments(arr, len(segs), B, col, ptr(out_v), None if want_idx64 else ptr(out_i),
+                                   ptr(out_i) if want_idx64 else None, ptr(cnt), stream()))
     return (out_v, out_i, cnt) if want_counts else (out_v, out_i)
 
 
@@ -461,7 +376,7 @@ def label_sample_proposals(prop_boxes, prop_count, gt, K, S, Fcap, iou_thresh, i
                            bump_rng=True, want_prelabels=False, want_index=False):
     """-> dict(boxes (B,S,4), valid (B,S) bool, classes (B,S) int64, gt_boxes, gt_boxes3D (B,S,9), gt_poses (B,S,3,3),
     stats (2,) [, index (B,S)] [, pre = (matched_idx, matched_iou, labels) each (B,P+G)])."""
-    L = _bind()
+    L = _lib.lib()
     B, P, _ = prop_boxes.shape
     G = gt["boxes"].shape[1]
     dev = prop_boxes.device
@@ -482,7 +397,7 @@ def label_sample_proposals(prop_boxes, prop_count, gt, K, S, Fcap, iou_thresh, i
     idx = torch.empty((B, S), dtype=torch.int64, device=dev) if want_index else None
     if rng is None:
         rng = rng_state(dev)
-    a = LabelSampleArgs()
+    a = _lib.LabelSampleArgs()
     a.prop_boxes, a.prop_count, a.gt_boxes, a.gt_classes, a.gt_present = pb.data_ptr(), pc.data_ptr(), gb.data_ptr(), gc.data_ptr(), pres.data_ptr()
     a.gt_boxes3D, a.gt_poses = g3.data_ptr(), gp.data_ptr()
     a.B, a.P, a.G, a.K, a.S, a.Fcap, a.append_gt = B, P, G, int(K), int(S), int(Fcap), int(bool(append_gt))
@@ -494,7 +409,7 @@ def label_sample_proposals(prop_boxes, prop_count, gt, K, S, Fcap, iou_thresh, i
     a.s_gt_boxes, a.s_gt_boxes3D, a.s_gt_poses = out["gt_boxes"].data_ptr(), out["gt_boxes3D"].data_ptr(), out["gt_poses"].data_ptr()
     a.s_index = idx.data_ptr() if idx is not None else None
     a.stats = out["stats"].data_ptr()
-    _lib.check(L.c3d_label_sample_proposals(ctypes.byref(a), _st()), launches=2 if bump_rng else 1)
+    _lib.check(L.c3d_label_sample_proposals(ctypes.byref(a), stream()), launches=2 if bump_rng else 1)
     out["valid"] = out["valid"].view(torch.bool)
     if idx is not None:
         out["index"] = idx
@@ -506,7 +421,7 @@ def label_sample_proposals(prop_boxes, prop_count, gt, K, S, Fcap, iou_thresh, i
 def anchor_sample(labels01, matched_iou, max_ioa, best_idx, gt_valid, gt_ign, n_total, cap_pos, ignore_thresh, rng=None,
                   bump_rng=True):
     """labels01 (B,A) int8 matcher labels {0,1} -> sampled labels (B,A) int8 in {-1,0,1} (rpn.py:62-105)."""
-    L = _bind()
+    L = _lib.lib()
     B, A = labels01.shape
     dev = labels01.device
     G = gt_valid.shape[1]
@@ -515,22 +430,22 @@ def anchor_sample(labels01, matched_iou, max_ioa, best_idx, gt_valid, gt_ign, n_
     keys = torch.empty((B, 2, A), dtype=torch.float32, device=dev)
     counts = torch.empty((B, 2), dtype=torch.int32, device=dev)
     lab = labels01.contiguous()
-    _lib.check(L.c3d_anchor_sample_keys(_p(lab), _p(matched_iou.contiguous()), B, A, _p(rng), _p(keys), _p(counts), _st()))
+    _lib.check(L.c3d_anchor_sample_keys(ptr(lab), ptr(matched_iou.contiguous()), B, A, ptr(rng), ptr(keys), ptr(counts), stream()))
     k = int(max(cap_pos, n_total))
     kv = keys.view(B, 2 * A)
     _, idx = topk_segments([(kv[:, :A], k), (kv[:, A:], k)])
     out = torch.empty((B, A), dtype=torch.int8, device=dev)
     v8, i8 = gt_valid.to(torch.uint8).contiguous(), gt_ign.to(torch.uint8).contiguous()
-    _lib.check(L.c3d_anchor_sample_finish(_p(lab), _p(max_ioa.contiguous()), _p(idx), _p(counts), _p(best_idx.contiguous()),
-                                          _p(v8), _p(i8), B, G, A, k, int(cap_pos), int(n_total), float(ignore_thresh),
-                                          _p(out), _p(rng) if bump_rng else None, _st()))
+    _lib.check(L.c3d_anchor_sample_finish(ptr(lab), ptr(max_ioa.contiguous()), ptr(idx), ptr(counts), ptr(best_idx.contiguous()),
+                                          ptr(v8), ptr(i8), B, G, A, k, int(cap_pos), int(n_total), float(ignore_thresh),
+                                          ptr(out), ptr(rng) if bump_rng else None, stream()))
     return out
 
 
 def det_candidates(probs, boxes, prop_count, image_hw, score_thresh):
     """probs (B,P,K+1), boxes (B,P,K,4) fp32 -> cand_score (B,P*K) (-inf = filtered), cand_boxes (B,P*K,4) clipped,
     maxc (B,), total (B,) int32 (fast_rcnn.py:76-100 for the whole batch)."""
-    L = _bind()
+    L = _lib.lib()
     B, P, K1 = probs.shape
     K = K1 - 1
     dev = probs.device
@@ -539,9 +454,9 @@ def det_candidates(probs, boxes, prop_count, image_hw, score_thresh):
     cb = torch.empty((B, P * K, 4), dtype=torch.float32, device=dev)
     maxc = torch.empty((B,), dtype=torch.float32, device=dev)
     total = torch.empty((B,), dtype=torch.int32, device=dev)
-    _lib.check(L.c3d_det_candidates(_p(probs), _p(boxes), _p(prop_count.to(torch.int32).contiguous()),
-                                    _p(image_hw.contiguous().float()), B, P, K, float(score_thresh), _p(cs), _p(cb), _p(maxc),
-                                    _p(total), _st()))
+    _lib.check(L.c3d_det_candidates(ptr(probs), ptr(boxes), ptr(prop_count.to(torch.int32).contiguous()),
+                                    ptr(image_hw.contiguous().float()), B, P, K, float(score_thresh), ptr(cs), ptr(cb), ptr(maxc),
+                                    ptr(total), stream()))
     return cs, cb, maxc, total
 
 
@@ -549,54 +464,54 @@ def det_candidates(probs, boxes, prop_count, image_hw, score_thresh):
 def box_loss_fwd(pred, classes, valid, boxes, gt_boxes, K, weights):
     """pred (R, ld) fp32 rows [K+1 scores | 4K deltas | pad] -> acc (8,) fp32 [sum CE, sum L1(fg), #valid, #fg, #correct,
     #fg correct, #fg predicted background, 0] (fast_rcnn.py:145-194)."""
-    L = _bind()
+    L = _lib.lib()
     R, ld = pred.shape
     acc = torch.empty(8, dtype=torch.float32, device=pred.device)
     w = (f32 * 4)(*[float(v) for v in weights])
-    _lib.check(L.c3d_box_loss_fwd(_p(pred), ld, _p(classes), _p(valid), _p(boxes), _p(gt_boxes), R, int(K), w, _p(acc), _st()))
+    _lib.check(L.c3d_box_loss_fwd(ptr(pred), ld, ptr(classes), ptr(valid), ptr(boxes), ptr(gt_boxes), R, int(K), w, ptr(acc), stream()))
     return acc
 
 
 def box_loss_bwd(pred, classes, valid, boxes, gt_boxes, K, weights, acc, g2):
-    L = _bind()
+    L = _lib.lib()
     R, ld = pred.shape
     dpred = torch.empty_like(pred)
     w = (f32 * 4)(*[float(v) for v in weights])
-    _lib.check(L.c3d_box_loss_bwd(_p(pred), ld, _p(classes), _p(valid), _p(boxes), _p(gt_boxes), R, int(K), w, _p(acc), _p(g2),
-                                  _p(dpred), _st()))
+    _lib.check(L.c3d_box_loss_bwd(ptr(pred), ld, ptr(classes), ptr(valid), ptr(boxes), ptr(gt_boxes), R, int(K), w, ptr(acc), ptr(g2),
+                                  ptr(dpred), stream()))
     return dpred
 
 
 def cube_gather(pred, classes, boxes, meta, priors, gt3, gtR, per_image, K, virtual_focal):
     """-> raw (n,13), aux (n,28): the inputs of c3d_cube_loss_fwd/bwd (roi_heads.py:372-461)."""
-    L = _bind()
+    L = _lib.lib()
     n, ld = pred.shape
     raw = torch.empty((n, 13), dtype=torch.float32, device=pred.device)
     aux = torch.empty((n, 28), dtype=torch.float32, device=pred.device)
-    _lib.check(L.c3d_cube_gather(_p(pred), ld, _p(classes), _p(boxes), _p(meta), _p(priors), _p(gt3), _p(gtR), n, int(per_image),
-                                 int(K), float(virtual_focal), _p(raw), _p(aux), _st()))
+    _lib.check(L.c3d_cube_gather(ptr(pred), ld, ptr(classes), ptr(boxes), ptr(meta), ptr(priors), ptr(gt3), ptr(gtR), n, int(per_image),
+                                 int(K), float(virtual_focal), ptr(raw), ptr(aux), stream()))
     return raw, aux
 
 
 def cube_reduce_fwd(rows, valid):
-    L = _bind()
+    L = _lib.lib()
     sums = torch.empty(12, dtype=torch.float32, device=rows.device)
     cnts = torch.empty(8, dtype=torch.float32, device=rows.device)
-    _lib.check(L.c3d_cube_reduce_fwd(_p(rows), _p(valid), rows.shape[0], _p(sums), _p(cnts), _st()))
+    _lib.check(L.c3d_cube_reduce_fwd(ptr(rows), ptr(valid), rows.shape[0], ptr(sums), ptr(cnts), stream()))
     return sums, cnts
 
 
 def cube_reduce_bwd(rows, valid, cnts, g6):
-    L = _bind()
+    L = _lib.lib()
     n = rows.shape[0]
     d = torch.empty((n, 6), dtype=torch.float32, device=rows.device)
-    _lib.check(L.c3d_cube_reduce_bwd(_p(rows), _p(valid), n, _p(cnts), _p(g6), _p(d), _st()))
+    _lib.check(L.c3d_cube_reduce_bwd(ptr(rows), ptr(valid), n, ptr(cnts), ptr(g6), ptr(d), stream()))
     return d
 
 
 def cube_scatter(draw, classes, K, ld):
-    L = _bind()
+    L = _lib.lib()
     n = draw.shape[0]
     dpred = torch.empty((n, ld), dtype=torch.float32, device=draw.device)
-    _lib.check(L.c3d_cube_scatter(_p(draw), _p(classes), n, int(K), int(ld), _p(dpred), _st()))
+    _lib.check(L.c3d_cube_scatter(ptr(draw), ptr(classes), n, int(K), int(ld), ptr(dpred), stream()))
     return dpred

@@ -6,12 +6,12 @@ kernels' bf16 OHWI layouts once per parameter version.  Forward AND backward run
   conv fwd  -> c3d_conv2d_fwd          dgrad -> c3d_conv2d_fwd with flipped/transposed weights
   wgrad     -> c3d_conv2d_wgrad        BN    -> c3d_bn_finalize / c3d_bn_apply / c3d_bn_bwd
 """
-import ctypes
 import os
 import weakref
 
 import torch
 
+from . import _lib
 from . import conv as K
 from . import kernels as Kx
 
@@ -60,12 +60,6 @@ _tap_index = {}
 _plans = {}
 
 
-class _PackDesc(ctypes.Structure):
-    _fields_ = [("src", ctypes.c_void_p), ("fwd", ctypes.c_void_p), ("dgrad", ctypes.c_void_p), ("phase", ctypes.c_void_p * 4),
-                ("start", ctypes.c_int64), ("Cout", ctypes.c_int32), ("Cin", ctypes.c_int32), ("KH", ctypes.c_int32),
-                ("KW", ctypes.c_int32), ("ohwi", ctypes.c_int32), ("pad_", ctypes.c_int32)]
-
-
 def prepack_model(model):
     """Pack every directly-used conv weight of `model` (forward OHWI pack, rotated data-gradient pack, and the four phase
     sub-kernels of 3x3 / stride-2 layers) with one kernel launch and seed the per-parameter caches, so the layer-by-layer
@@ -79,7 +73,7 @@ def prepack_model(model):
     plan = _plans.get(id(model))
     if plan is None or plan["key"] != key:
         dev = convs[0].weight.device
-        arr = (_PackDesc * len(convs))()
+        arr = (_lib.PackDesc * len(convs))()
         bufs, start = [], 0
         for i, m in enumerate(convs):
             w = m.weight
@@ -102,18 +96,12 @@ def prepack_model(model):
             for a in (0, 1):
                 for b in (0, 1):
                     d.phase[a * 2 + b] = ph[(a, b)].data_ptr() if ph else None
-            d.start, d.Cout, d.Cin, d.KH, d.KW, d.ohwi, d.pad_ = start, O, I, KH, KW, int(ohwi), int(bool(merged))
+            d.start, d.Cout, d.Cin, d.KH, d.KW, d.src_is_ohwi, d.merged_phases = start, O, I, KH, KW, int(ohwi), int(bool(merged))
             start += w.numel()
             bufs.append((w, f, g, ph))
         table = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
         plan = _plans[id(model)] = {"key": key, "table": table, "bufs": bufs, "total": start, "n": len(convs)}
-    L = K._bind()
-    if not hasattr(L, "_c3d_pack_bound"):
-        L.c3d_pack_conv_weights_batched.restype = ctypes.c_int32
-        L.c3d_pack_conv_weights_batched.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p]
-        L._c3d_pack_bound = True
-    from . import _lib
-    _lib.check(L.c3d_pack_conv_weights_batched(plan["table"].data_ptr(), plan["n"], plan["total"], K._stream()))
+    _lib.check(_lib.lib().c3d_pack_conv_weights_batched(plan["table"].data_ptr(), plan["n"], plan["total"], _lib.stream()))
     for w, f, g, ph in plan["bufs"]:
         k, ver = _cache_key(w)
         _pack_cache[k] = (ver, f, g, weakref.ref(w))

@@ -1,36 +1,130 @@
-"""CPU test: libc3d.so loads and exports every symbol include/c3d.h declares (no compute calls)."""
+"""CPU tests of the C ABI: include/c3d.h against libc3d.so and the ctypes declarations of omni3d_b200/_lib.py (prototypes,
+struct layouts), plus the entry points that only do host arithmetic or argument checking (no compute calls)."""
 import ctypes
 import os
 import re
+import shutil
+import subprocess
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = os.path.join(ROOT, "include", "c3d.h")
+
+# by-value C types of the ABI and the ctypes type each must be bound as
+_SCALARS = {"int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64, "size_t": ctypes.c_size_t, "float": ctypes.c_float,
+            "double": ctypes.c_double}
 
 
-def _declared():
-    names = set()
-    for f in os.listdir(os.path.join(ROOT, "include")):
-        if f.endswith(".h"):
-            src = open(os.path.join(ROOT, "include", f)).read()
-            src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-            names |= set(re.findall(r"\b(c3d_[a-z0-9_]+)\s*\(", src))
-    return sorted(names)
+def _header_source():
+    src = open(HEADER).read()
+    src = re.sub(r"/\*.*?\*/", " ", src, flags=re.S)
+    src = re.sub(r"//[^\n]*", " ", src)
+    return re.sub(r"^\s*#[^\n]*", " ", src, flags=re.M)
 
 
-def test_library_exports_every_declared_symbol():
+def _c_type(decl, named=False):
+    """'const float* boxes' -> ('float', 1); named: the declaration ends in a parameter name."""
+    toks = [t for t in re.findall(r"\w+|\*", decl) if t != "const"]
+    if named:
+        assert len(toks) >= 2 and toks[-1] != "*", f"unnamed parameter {decl!r}"
+        toks = toks[:-1]
+    assert toks and toks[0] != "*" and all(t == "*" for t in toks[1:]), f"unparsed type {decl!r}"
+    return toks[0], len(toks) - 1
+
+
+def _prototypes():
+    """{name: (return type, [parameter types])} of every c3d_* function c3d.h declares."""
+    src = _header_source()
+    protos = {}
+    for stmt in re.split(r"[;{}]", src):
+        m = re.fullmatch(r"\s*([\w\s*]+?)\s*\b(c3d_\w+)\s*\(([^()]*)\)\s*", stmt)
+        if m:
+            ret, name, params = m.groups()
+            params = [] if params.strip() == "void" else [_c_type(p, named=True) for p in params.split(",")]
+            protos[name] = (_c_type(ret), params)
+    # a declaration this parser missed would drop out of every check below
+    assert set(protos) == set(re.findall(r"\b(c3d_\w+)\s*\(", src)), "c3d.h declaration the prototype parser missed"
+    return protos
+
+
+def _expected_ctype(base, depth):
+    from omni3d_b200 import _lib
+    if depth == 0:
+        assert base in _SCALARS, f"by-value {base} has no ctypes mapping"
+        return _SCALARS[base]
+    if base == "char":
+        return ctypes.c_char_p
+    if base in _lib.STRUCTS:
+        assert depth == 1, f"{base} passed through {depth} pointer levels"
+        return ctypes.POINTER(_lib.STRUCTS[base])
+    return ctypes.c_void_p
+
+
+def _lib_path():
     from omni3d_b200 import _lib
     if not os.path.exists(_lib.LIB_PATH):
         import __graft_entry__
         __graft_entry__.build()
-    L = ctypes.CDLL(_lib.LIB_PATH)
-    decl = _declared()
-    assert len(decl) >= 6
-    for name in decl:
-        assert hasattr(L, name), f"{name} declared in include/*.h but not exported"
-    assert sorted(_lib.EXPORTS) == decl, "omni3d_b200/_lib.py EXPORTS out of sync with include/c3d.h"
-    L.c3d_abi_version.restype = ctypes.c_int32
-    assert L.c3d_abi_version() >= 1
+    return _lib.LIB_PATH
+
+
+def test_bindings_match_header_prototypes():
+    """every c3d.h prototype is exported by the library and bound in _lib.SIGNATURES with the same arity, argument types
+    and return type; nothing else is bound."""
+    from omni3d_b200 import _lib
+    protos = _prototypes()
+    assert len(protos) >= 6
+    unbound, undeclared = sorted(set(protos) - set(_lib.SIGNATURES)), sorted(set(_lib.SIGNATURES) - set(protos))
+    assert not unbound and not undeclared, \
+        f"declared in include/c3d.h but not in _lib.SIGNATURES: {unbound}; in _lib.SIGNATURES but not declared: {undeclared}"
+    so = ctypes.CDLL(_lib_path())
+    missing = [name for name in protos if not hasattr(so, name)]
+    assert not missing, f"declared in include/c3d.h but not exported by libc3d.so: {missing}"
+    bad = []
+    for name, (ret, params) in protos.items():
+        bound_ret, bound_params = _lib.SIGNATURES[name]
+        if bound_ret is not _expected_ctype(*ret):
+            bad.append(f"{name}: returns {ret}, bound as {bound_ret.__name__}")
+        if len(bound_params) != len(params):
+            bad.append(f"{name}: {len(params)} parameters, bound with {len(bound_params)}")
+            continue
+        for i, (p, t) in enumerate(zip(params, bound_params)):
+            if t is not _expected_ctype(*p):
+                bad.append(f"{name} parameter {i}: {p}, bound as {t.__name__}")
+    assert not bad, "\n".join(bad)
+    assert _lib.lib().c3d_abi_version() >= 1
+
+
+def test_struct_mirrors_match_header_layout(tmp_path):
+    """sizeof and every field's offset / size of the ctypes mirrors equal what the C compiler makes of c3d.h."""
+    from omni3d_b200 import _lib
+    cc = shutil.which("cc")
+    assert cc, "no host C compiler `cc` on PATH"
+    body = []
+    for cname, mirror in _lib.STRUCTS.items():
+        body.append(f'  printf("{cname} sizeof %zu\\n", sizeof({cname}));')
+        for f, _ in mirror._fields_:
+            body.append(f'  printf("{cname} {f} %zu %zu\\n", offsetof({cname}, {f}), sizeof((({cname}*)0)->{f}));')
+    src, exe = tmp_path / "layout.c", tmp_path / "layout"
+    src.write_text("#include <stddef.h>\n#include <stdio.h>\n#include \"c3d.h\"\nint main(void) {\n" + "\n".join(body)
+                   + "\n  return 0;\n}\n")
+    r = subprocess.run([cc, "-std=c99", "-I", os.path.dirname(HEADER), str(src), "-o", str(exe)], capture_output=True,
+                       text=True)
+    assert r.returncode == 0, f"layout probe does not compile against c3d.h:\n{r.stderr}"
+    layout = {}
+    for line in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.splitlines():
+        cname, field, *vals = line.split()
+        layout[cname, field] = tuple(int(v) for v in vals)
+    bad = []
+    for cname, mirror in _lib.STRUCTS.items():
+        if (ctypes.sizeof(mirror),) != layout[cname, "sizeof"]:
+            bad.append(f"sizeof({cname}) = {layout[cname, 'sizeof'][0]}, {mirror.__name__} has {ctypes.sizeof(mirror)}")
+        for f, _ in mirror._fields_:
+            got = (getattr(mirror, f).offset, getattr(mirror, f).size)
+            if got != layout[cname, f]:
+                bad.append(f"{cname}.{f} at (offset, size) {layout[cname, f]}, {mirror.__name__}.{f} at {got}")
+    assert not bad, "\n".join(bad)
 
 
 def test_product_fails_loudly_without_gpu():
@@ -57,24 +151,14 @@ def test_host_side_entry_points_without_gpu():
     """entry points that do host arithmetic or argument checking only: tile query (incl. the rolling-halo path's
     one-row-per-CTA statistics layout), workspace sizes, EINVAL + c3d_last_error on bad arguments (no CUDA call)."""
     from omni3d_b200 import _lib, conv
-    L = conv._bind()
-    d = conv.ConvDesc(32, 640, 640, 16, 16, 3, 3, 1, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)       # DLA level0: halo path
-    t, th, tw = conv.num_tiles(d)
-    if os.environ.get("C3D_CONV_NO_HALO"):
-        assert t == 32 * 640 * 640 // (th * tw)
-    else:
-        assert (t, th, tw) == (132 * 3, 1, 128)
-    d = conv.ConvDesc(32, 160, 160, 256, 256, 3, 3, 1, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)     # FPN output conv
+    L = _lib.lib()
+    d = _lib.ConvDesc(N=32, H=640, W=640, Cin=16, Cout=16, KH=3, KW=3, stride=1, pad=1)       # DLA level0: halo path
+    assert conv.num_tiles(d) == (132 * 3, 1, 128)
+    d = _lib.ConvDesc(N=32, H=160, W=160, Cin=256, Cout=256, KH=3, KW=3, stride=1, pad=1)     # FPN output conv
     t, th, tw = conv.num_tiles(d)
     assert th * tw <= 128 and t == 32 * -(-160 // th) * -(-160 // tw)
-    L.c3d_nms_workspace_bytes.restype = ctypes.c_size_t
-    L.c3d_nms_workspace_bytes.argtypes = [ctypes.c_int32, ctypes.c_int32]
     assert L.c3d_nms_workspace_bytes(32, 8192) > L.c3d_nms_workspace_bytes(32, 4096) > 32 * 4096 * 64 * 8
-    L.c3d_anchor_match.restype = ctypes.c_int32
-    L.c3d_last_error.restype = ctypes.c_char_p
     null = ctypes.c_void_p(None)
-    L.c3d_anchor_match.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
-                                   ctypes.c_int32, ctypes.c_int32, ctypes.c_float] + [ctypes.c_void_p] * 7
     rc = L.c3d_anchor_match(null, 10, null, null, null, 1, 1, 0.7, null, null, null, null, null, null, null)
     assert rc != 0 and b"anchor_match" in L.c3d_last_error()
     with pytest.raises(_lib.C3DError):
@@ -84,23 +168,21 @@ def test_host_side_entry_points_without_gpu():
 def test_conv_descriptor_argument_checks_without_gpu():
     """c3d_conv2d_fwd validates the descriptor before any CUDA call: odd outputs have no nearest-x2 addend, the in-place
     accumulate needs a bf16 output, the split channel placement needs a multiple of 16 and excludes addend / statistics."""
-    from omni3d_b200 import _lib, conv
-    L = conv._bind()
-    L.c3d_last_error.restype = ctypes.c_char_p
+    from omni3d_b200 import _lib
+    L = _lib.lib()
     p = ctypes.c_void_p(256)                       # non-null dummies: every case below is rejected before they are used
 
     def call(d, addend=p, stats=None):
         return L.c3d_conv2d_fwd(ctypes.byref(d), p, p, None, addend, p, stats, None)
 
-    d = conv.ConvDesc(2, 9, 11, 64, 64, 3, 3, 1, 1, 0, 0, 2, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)           # up2 addend, 9 x 11 output
-    assert call(d) == _lib.C3D_EINVAL and b"even output" in L.c3d_last_error()
-    d = conv.ConvDesc(2, 8, 8, 64, 64, 3, 3, 1, 1, 0, 0, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)             # addend mode without addend
-    assert call(d, addend=None) == _lib.C3D_EINVAL and b"addend missing" in L.c3d_last_error()
-    d = conv.ConvDesc(2, 8, 8, 64, 64, 3, 3, 1, 1, 0, 1, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)             # accumulate into fp32
-    assert call(d) == _lib.C3D_EINVAL and b"bf16 output" in L.c3d_last_error()
-    d = conv.ConvDesc(2, 8, 8, 64, 64, 2, 2, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 8, 8, 0, 24, 0, 100)           # split not a multiple of 16
+    def desc(**kw):                                # a 3x3 conv of 2 x 8 x 8 x 64 unless kw says otherwise
+        return _lib.ConvDesc(**{**dict(N=2, H=8, W=8, Cin=64, Cout=64, KH=3, KW=3, stride=1, pad=1), **kw})
+
+    assert call(desc(H=9, W=11, add_mode=2)) == _lib.C3D_EINVAL and b"even output" in L.c3d_last_error()   # up2, 9 x 11 output
+    assert call(desc(add_mode=1), addend=None) == _lib.C3D_EINVAL and b"addend missing" in L.c3d_last_error()
+    assert call(desc(out_fp32=1, add_mode=3)) == _lib.C3D_EINVAL and b"bf16 output" in L.c3d_last_error()  # accumulate into fp32
+    d = desc(KH=2, KW=2, pad=0, out_h=8, out_w=8, y_split_c=24, y_split_off=100)                     # split not a multiple of 16
     assert call(d, addend=None) == _lib.C3D_EINVAL and b"y_split_c" in L.c3d_last_error()
-    d = conv.ConvDesc(2, 8, 8, 64, 64, 3, 3, 3, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0)             # stride 3
-    assert call(d, addend=None) == _lib.C3D_EINVAL and b"stride" in L.c3d_last_error()
+    assert call(desc(stride=3), addend=None) == _lib.C3D_EINVAL and b"stride" in L.c3d_last_error()
     with pytest.raises(_lib.C3DError):
         _lib.check(_lib.C3D_EINVAL)

@@ -9,7 +9,7 @@ import torch
 from omni3d_b200 import conv as K
 from omni3d_b200 import nnfunc
 
-STEM_C = 16 if os.environ.get("C3D_CONV_NO_HALO") else 8     # NHWC8 image for the rolling-halo stem kernel
+STEM_C = 8     # NHWC8 image for the rolling-halo stem kernel
 SHAPES = [  # name, H, W, Cin, Cout, k, stride, pad, real_cin, count in DLA34_FPN (+RPN head), has_dgrad
     ("stem7x7_3(%d)->16@640" % STEM_C, 640, 640, STEM_C, 16, 7, 1, 3, 3, 1, False),
     ("level0_16->16@640", 640, 640, 16, 16, 3, 1, 1, 16, 1, True),
