@@ -128,22 +128,26 @@ int32_t c3d_conv2d_wgrad(const c3d_conv_desc* d, const void* x, const void* dy, 
  * optimizer's gradient arena, no layout conversion pass) */
 int32_t c3d_conv2d_wgrad_ex(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int32_t oihw,
                             void* stream);
-/* fp32 master weight (OIHW, or OHWI = torch channels_last storage when src_is_ohwi != 0) -> bf16 (Cout,KH,KW,Cin)
- * forward pack and/or bf16 (Cin,KH,KW,Cout) 180-degree-rotated data-gradient pack (either output may be NULL) */
-int32_t c3d_pack_conv_weight(const float* w, int32_t Cout, int32_t Cin, int32_t KH, int32_t KW, int32_t src_is_ohwi,
-                             void* fwd_ohwi, void* dgrad_ihwo, void* stream);
-
-/* every conv weight of a model in one launch: descs_dev = device array of n c3d_pack_desc (forward pack, rotated /
- * transposed data-gradient pack and, for 3x3 stride-2 layers, the four phase sub-kernels of the phase-decomposed data
- * gradient: (Cin, KH', KW', Cout) with parity 0 -> tap [1], parity 1 -> taps [2, 0]); `start` = prefix sum of elements.
+/* Re-pack of one fp32 master conv weight src (Cout,Cin,KH,KW) — stored OIHW, or OHWI = torch channels_last storage when
+ * src_is_ohwi != 0 — into any of these bf16 outputs (NULL = not written):
+ *   fwd    (Cout,KH,KW,Cin) forward pack;
+ *   dgrad  (Cin,KH,KW,Cout) 180-degree-rotated data-gradient pack;
+ *   phase  the four sub-kernels of a 3x3 stride-2 layer's phase-decomposed data gradient, (Cin, KH', KW', Cout) with
+ *          parity 0 -> tap [1], parity 1 -> taps [2, 0]; all four or none.
  * merged_phases != 0: phase[(a,b) = 2*a+b] are the four row blocks [(2*a+b)*Cin, +Cin) of ONE (4*Cin, 2, 2, Cout) weight
  * (the merged stride-2 data gradient, see y_split_* of c3d_conv_desc): every phase is stored as 2x2 and the taps it does
- * not use are left untouched (the caller zeroes them once). */
+ * not use are left untouched (the caller zeroes them once).
+ * start: first element of this weight in the flat element range of c3d_pack_conv_weights_batched (prefix sum). */
 typedef struct {
   const float* src; void* fwd; void* dgrad; void* phase[4];
   int64_t start;
   int32_t Cout, Cin, KH, KW, src_is_ohwi, merged_phases;
 } c3d_pack_desc;
+/* one weight: *desc_host is read on the host and passed in the kernel parameters (no host->device copy, so the call can be
+ * recorded in a CUDA graph); `start` is ignored.  C3D_EINVAL for a NULL src, no output, a negative size, or phase outputs
+ * that are not all four or belong to a weight that is not 3x3. */
+int32_t c3d_pack_conv_weight(const c3d_pack_desc* desc_host, void* stream);
+/* every conv weight of a model in one launch: descs_dev = device array of n c3d_pack_desc, ordered by `start` */
 int32_t c3d_pack_conv_weights_batched(const void* descs_dev, int32_t n, int64_t total_elems, void* stream);
 
 /* ------------------------------------------------------------------------------------------
@@ -232,17 +236,12 @@ int32_t c3d_maxpool2_bwd_acc(const void* x, const void* dy, void* dx, int32_t N,
 int32_t c3d_maxpool3s2_fwd(const void* x, void* y, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
 int32_t c3d_maxpool3s2_bwd(const void* x, const void* dy, void* dx, int32_t N, int32_t H, int32_t W, int32_t C,
                            int64_t dy_stride, void* stream);
-/* (3,H,W) fp32 BGR image -> (Hp,Wp,Cp) bf16 NHWC slot: (x-mean)/std in channels 0..2, zeros elsewhere */
-int32_t c3d_preprocess_image(const float* img, int32_t H, int32_t W, void* out_slot, int32_t Hp, int32_t Wp,
-                             int32_t Cp, const float* mean3_host, const float* std3_host, void* stream);
-/* all N images of a batch in one launch: imgs_host / H_host / W_host are HOST arrays (device pointers, sizes) that travel in
- * the kernel parameters; out = (N,Hp,Wp,Cp) bf16; is_u8 selects uint8 or fp32 (3,H,W) inputs */
+/* (3,H,W) BGR images -> (N,Hp,Wp,Cp) bf16 NHWC slots: (x-mean)/std in channels 0..2, zeros elsewhere; all N images in one
+ * launch.  imgs_host / H_host / W_host are HOST arrays (device pointers, sizes) that travel in the kernel parameters;
+ * is_u8 selects uint8 inputs (the image tensor detectron2's DatasetMapper produces, dataset_mapper.py) or fp32 ones */
 int32_t c3d_preprocess_batch(const void* const* imgs_host, const int32_t* H_host, const int32_t* W_host, int32_t N,
                              int32_t is_u8, void* out, int32_t Hp, int32_t Wp, int32_t Cp, const float* mean3_host,
                              const float* std3_host, void* stream);
-/* same for the uint8 (3,H,W) image tensor detectron2's DatasetMapper produces (dataset_mapper.py: image as uint8) */
-int32_t c3d_preprocess_image_u8(const uint8_t* img, int32_t H, int32_t W, void* out_slot, int32_t Hp, int32_t Wp,
-                                int32_t Cp, const float* mean3_host, const float* std3_host, void* stream);
 /* flag |= 1 if any gradient element is NaN/Inf */
 int32_t c3d_grad_finite(const float* g, int64_t n, int32_t* flag, void* stream);
 /* torch.optim.SGD(momentum, weight_decay) over a flat arena; no-op if *skip_flag != 0 */

@@ -74,7 +74,7 @@ SIGNATURES = {
     "c3d_conv2d_fwd": (i32, [_conv, vp, vp, vp, vp, vp, vp, vp]),
     "c3d_conv2d_wgrad": (i32, [_conv, vp, vp, vp, vp]),
     "c3d_conv2d_wgrad_ex": (i32, [_conv, vp, vp, vp, i32, vp]),
-    "c3d_pack_conv_weight": (i32, [vp, i32, i32, i32, i32, i32, vp, vp, vp]),
+    "c3d_pack_conv_weight": (i32, [ctypes.POINTER(PackDesc), vp]),
     "c3d_pack_conv_weights_batched": (i32, [vp, i32, i64, vp]),
     # fully-connected layers
     "c3d_pack_linear_weight": (i32, [vp, i32, i32, i32, i32, vp, vp, vp]),
@@ -98,9 +98,7 @@ SIGNATURES = {
     "c3d_maxpool2_bwd_acc": (i32, [vp, vp, vp, i32, i32, i32, i32, i64, i64, i64, vp]),
     "c3d_maxpool3s2_fwd": (i32, [vp, vp, i32, i32, i32, i32, vp]),
     "c3d_maxpool3s2_bwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i64, vp]),
-    "c3d_preprocess_image": (i32, [vp, i32, i32, vp, i32, i32, i32, vp, vp, vp]),
     "c3d_preprocess_batch": (i32, [vp, vp, vp, i32, i32, vp, i32, i32, i32, vp, vp, vp]),
-    "c3d_preprocess_image_u8": (i32, [vp, i32, i32, vp, i32, i32, i32, vp, vp, vp]),
     "c3d_grad_finite": (i32, [vp, i64, vp, vp]),
     "c3d_sgd_momentum": (i32, [vp, vp, vp, i64, f32, f32, f32, f32, vp, vp]),
     "c3d_sgd_momentum_dev": (i32, [vp, vp, vp, i64, vp, f32, f32, f32, vp, vp]),

@@ -74,18 +74,41 @@ def conv2d_fwd(x, w, bias=None, stride=1, pad=0, relu=False, addend=None, up2=Fa
     return (out, stats) if want_stats else out
 
 
-def pack_conv_weight(w, want_fwd=True, want_dgrad=True):
-    """fp32 (Cout,Cin,KH,KW) -> bf16 (Cout,KH,KW,Cin) and bf16 (Cin,KH,KW,Cout) rotated, in ONE launch."""
-    L = _lib.lib()
+def pack_desc(w, want_fwd=True, want_dgrad=True, phases=None):
+    """c3d_pack_desc of the fp32 master w (Cout,Cin,KH,KW), stored OIHW or channels_last, and the new bf16 outputs it points
+    at -> (desc, (fwd, dgrad, phase packs)).  fwd (Cout,KH,KW,Cin); dgrad (Cin,KH,KW,Cout) rotated by 180 degrees; phases
+    of a 3x3 weight: "separate" -> {(a, b): (Cin, 1 + a, 1 + b, Cout)}, "merged" -> the same keys as the row blocks of
+    packs["merged"], one zeroed (4*Cin, 2, 2, Cout) weight whose unused taps the pack never writes (include/c3d.h)."""
     Cout, Cin, KH, KW = w.shape
+    ohwi = (not w.is_contiguous()) and w.permute(0, 2, 3, 1).is_contiguous()
+    if not (ohwi or w.is_contiguous()):
+        raise ValueError("conv weight storage is neither OIHW nor channels_last")
+    new = lambda *shape: torch.empty(shape, device=w.device, dtype=torch.bfloat16)
+    f = new(Cout, KH, KW, Cin) if want_fwd else None
+    g = new(Cin, KH, KW, Cout) if want_dgrad else None
+    ph = None
+    if phases == "merged":
+        mg = torch.zeros((4 * Cin, 2, 2, Cout), device=w.device, dtype=torch.bfloat16)
+        ph = {"merged": mg, **{(a, b): mg[(2 * a + b) * Cin:(2 * a + b + 1) * Cin] for a in (0, 1) for b in (0, 1)}}
+    elif phases == "separate":
+        ph = {(a, b): new(Cin, 1 + a, 1 + b, Cout) for a in (0, 1) for b in (0, 1)}
+    elif phases is not None:
+        raise ValueError(f"phases must be None, 'separate' or 'merged', not {phases!r}")
+    d = _lib.PackDesc(src=w.data_ptr(), fwd=ptr(f), dgrad=ptr(g), Cout=Cout, Cin=Cin, KH=KH, KW=KW, src_is_ohwi=int(ohwi),
+                      merged_phases=int(phases == "merged"))
+    if ph is not None:
+        d.phase = (ctypes.c_void_p * 4)(*[ph[(a, b)].data_ptr() for a in (0, 1) for b in (0, 1)])
+    return d, (f, g, ph)
+
+
+def pack_conv_weight(w, want_fwd=True, want_dgrad=True, phases=None):
+    """fp32 (Cout,Cin,KH,KW) -> (bf16 fwd, bf16 dgrad, stride-2 phase packs | None) of pack_desc, in ONE launch."""
     w = w.detach()
-    ohwi = (not w.is_contiguous()) and w.permute(0, 2, 3, 1).is_contiguous()     # channels_last master storage
-    if not ohwi:
+    if not (w.is_contiguous() or w.permute(0, 2, 3, 1).is_contiguous()):
         w = w.contiguous()
-    f = torch.empty((Cout, KH, KW, Cin), device=w.device, dtype=torch.bfloat16) if want_fwd else None
-    g = torch.empty((Cin, KH, KW, Cout), device=w.device, dtype=torch.bfloat16) if want_dgrad else None
-    _lib.check(L.c3d_pack_conv_weight(ptr(w), Cout, Cin, KH, KW, int(ohwi), ptr(f), ptr(g), stream()))
-    return f, g
+    d, packs = pack_desc(w, want_fwd, want_dgrad, phases)
+    _lib.check(_lib.lib().c3d_pack_conv_weight(ctypes.byref(d), stream()))
+    return packs
 
 
 def conv2d_wgrad(x, dy, KH, KW, stride=1, pad=0, dw=None, oihw=False):

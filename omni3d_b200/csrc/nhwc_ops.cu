@@ -560,90 +560,50 @@ __global__ void maxpool3s2_bwd_kernel(const bf16* __restrict__ x, const bf16* __
   }
 }
 
-// ---- weight re-pack: fp32 OIHW master -> bf16 OHWI (forward) and bf16 rotated/transposed (data gradient) ----
-__global__ void pack_conv_weight_kernel(const float* __restrict__ w, int Cout, int Cin, int KH, int KW, int src_ohwi,
-                                        bf16* __restrict__ fwd, bf16* __restrict__ dgrad) {
-  const long long total = (long long)Cout * Cin * KH * KW;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    int kw, kh, ci, co;
-    if (src_ohwi) {                      // master stored (Cout,KH,KW,Cin): the forward pack is a plain cast
-      ci = (int)(i % Cin);
-      long long t = i / Cin;
-      kw = (int)(t % KW); t /= KW;
-      kh = (int)(t % KH);
-      co = (int)(t / KH);
-    } else {
-      kw = (int)(i % KW);
-      long long t = i / KW;
-      kh = (int)(t % KH); t /= KH;
-      ci = (int)(t % Cin);
-      co = (int)(t / Cin);
-    }
-    const bf16 v = __float2bfloat16(w[i]);
-    if (fwd) fwd[(((long long)co * KH + kh) * KW + kw) * Cin + ci] = v;
-    if (dgrad) dgrad[(((long long)ci * KH + (KH - 1 - kh)) * KW + (KW - 1 - kw)) * Cout + co] = v;
+// ---- weight re-pack: fp32 OIHW / OHWI master -> bf16 OHWI (forward), bf16 rotated/transposed (data gradient) and the
+// stride-2 phase sub-kernels (include/c3d.h c3d_pack_desc) ----
+// Element i of D's source writes its forward-pack entry, its rotated / transposed data-gradient entry and — for 3x3
+// stride-2 layers — its entry in the phase sub-kernel it belongs to (parity 0 uses tap [1], parity 1 taps [2, 0]).
+__device__ __forceinline__ void pack_conv_weight_element(const c3d_pack_desc& D, long long i) {
+  int kw, kh, ci, co;
+  if (D.src_is_ohwi) {
+    ci = (int)(i % D.Cin); long long t = i / D.Cin;
+    kw = (int)(t % D.KW); t /= D.KW;
+    kh = (int)(t % D.KH); co = (int)(t / D.KH);
+  } else {
+    kw = (int)(i % D.KW); long long t = i / D.KW;
+    kh = (int)(t % D.KH); t /= D.KH;
+    ci = (int)(t % D.Cin); co = (int)(t / D.Cin);
+  }
+  const bf16 v = __float2bfloat16(D.src[i]);
+  if (D.fwd) static_cast<bf16*>(D.fwd)[(((long long)co * D.KH + kh) * D.KW + kw) * D.Cin + ci] = v;
+  if (D.dgrad) static_cast<bf16*>(D.dgrad)[(((long long)ci * D.KH + (D.KH - 1 - kh)) * D.KW + (D.KW - 1 - kw)) * D.Cout + co] = v;
+  if (D.phase[0]) {               // 3x3 only: parity a = (kh != 1), position inside the phase: kh 1 -> 0 | kh 2 -> 0, kh 0 -> 1
+    const int a = kh != 1, b = kw != 1;
+    const int ph = a ? (kh == 2 ? 0 : 1) : 0, pw = b ? (kw == 2 ? 0 : 1) : 0;
+    // merged_phases: every phase is a 2x2 row block of one (4*Cin, 2, 2, Cout) weight (include/c3d.h c3d_pack_desc)
+    const int KHp = (a || D.merged_phases) ? 2 : 1, KWp = (b || D.merged_phases) ? 2 : 1;
+    static_cast<bf16*>(D.phase[a * 2 + b])[(((long long)ci * KHp + ph) * KWp + pw) * D.Cout + co] = v;
   }
 }
 
-// All conv weights of the model in ONE launch (the per-parameter kernel above ran 58 times per step + ~70 ATen launches for the
-// stride-2 phase sub-kernels): every source element writes its forward-pack entry, its rotated / transposed data-gradient
-// entry and — for 3x3 stride-2 layers — its entry in the phase sub-kernel it belongs to (nnfunc._phase_packs:
-// parity 0 uses tap [1], parity 1 taps [2, 0]).
+// one weight; the descriptor travels in the kernel parameters (no host->device copy: the launch can be graph-captured)
+__global__ void pack_conv_weight_desc_kernel(const c3d_pack_desc D, long long total) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
+    pack_conv_weight_element(D, i);
+}
+
+// every conv weight of a model in ONE launch: element e belongs to the descriptor with the last start <= e
 __global__ void pack_conv_weights_batched_kernel(const c3d_pack_desc* __restrict__ descs, int n, long long total) {
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     int lo = 0, hi = n;
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (descs[mid].start <= e) lo = mid; else hi = mid; }
     const c3d_pack_desc D = descs[lo];
-    const long long i = e - D.start;
-    int kw, kh, ci, co;
-    if (D.src_is_ohwi) {
-      ci = (int)(i % D.Cin); long long t = i / D.Cin;
-      kw = (int)(t % D.KW); t /= D.KW;
-      kh = (int)(t % D.KH); co = (int)(t / D.KH);
-    } else {
-      kw = (int)(i % D.KW); long long t = i / D.KW;
-      kh = (int)(t % D.KH); t /= D.KH;
-      ci = (int)(t % D.Cin); co = (int)(t / D.Cin);
-    }
-    const bf16 v = __float2bfloat16(D.src[i]);
-    if (D.fwd) static_cast<bf16*>(D.fwd)[(((long long)co * D.KH + kh) * D.KW + kw) * D.Cin + ci] = v;
-    if (D.dgrad) static_cast<bf16*>(D.dgrad)[(((long long)ci * D.KH + (D.KH - 1 - kh)) * D.KW + (D.KW - 1 - kw)) * D.Cout + co] = v;
-    if (D.phase[0]) {               // 3x3 only: parity a = (kh != 1), position inside the phase: kh 1 -> 0 | kh 2 -> 0, kh 0 -> 1
-      const int a = kh != 1, b = kw != 1;
-      const int ph = a ? (kh == 2 ? 0 : 1) : 0, pw = b ? (kw == 2 ? 0 : 1) : 0;
-      // merged_phases: every phase is a 2x2 row block of one (4*Cin, 2, 2, Cout) weight (include/c3d.h c3d_pack_desc)
-      const int KHp = (a || D.merged_phases) ? 2 : 1, KWp = (b || D.merged_phases) ? 2 : 1;
-      static_cast<bf16*>(D.phase[a * 2 + b])[(((long long)ci * KHp + ph) * KWp + pw) * D.Cout + co] = v;
-    }
+    pack_conv_weight_element(D, e - D.start);
   }
 }
 
-// ---- image normalisation: (3,H,W) fp32 BGR -> (Hp,Wp,Cp) bf16 NHWC slot, zero padded --------------
-template <typename T>
-__global__ void preprocess_kernel(const T* __restrict__ img, int H, int W, bf16* __restrict__ out, int Hp,
-                                  int Wp, int Cp, float m0, float m1, float m2, float s0, float s1, float s2) {
-  const long long total = (long long)Hp * Wp;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int w = (int)(i % Wp), h = (int)(i / Wp);
-    float v0 = 0.f, v1 = 0.f, v2 = 0.f;
-    if (h < H && w < W) {
-      const long long o = (long long)h * W + w;
-      v0 = ((float)img[o] - m0) / s0;
-      v1 = ((float)img[(long long)H * W + o] - m1) / s1;
-      v2 = ((float)img[2LL * H * W + o] - m2) / s2;
-    }
-    bf16* dst = out + i * Cp;
-    for (int c = 0; c < Cp; c += 8) {
-      V8 z;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) z.v[k] = 0.f;
-      if (c == 0) { z.v[0] = v0; z.v[1] = v1; z.v[2] = v2; }
-      st8(dst + c, z);
-    }
-  }
-}
-
+// ---- image normalisation: (3,H,W) fp32 / uint8 BGR -> (Hp,Wp,Cp) bf16 NHWC slots, zero padded -------------
 // all images of a batch in ONE launch (blockIdx.y = image; pointers and sizes travel in the kernel parameters)
 constexpr int kPreBatch = 64;
 struct PreBatch { const void* img[kPreBatch]; int H[kPreBatch]; int W[kPreBatch]; };
@@ -812,24 +772,6 @@ extern "C" int32_t c3d_maxpool3s2_bwd(const void* x, const void* dy, void* dx, i
                                                                                N, H, W, C, dy_stride ? dy_stride : C);
   return check_launch("maxpool3s2_bwd");
 }
-extern "C" int32_t c3d_preprocess_image(const float* img, int32_t H, int32_t W, void* out_slot, int32_t Hp,
-                                        int32_t Wp, int32_t Cp, const float* mean3_host, const float* std3_host,
-                                        void* stream) {
-  C3D_REQ(img && out_slot && mean3_host && std3_host && Cp % 8 == 0 && Hp >= H && Wp >= W, "preprocess: bad args");
-  preprocess_kernel<float><<<grid_for((long long)Hp * Wp, 256), 256, 0, (cudaStream_t)stream>>>(
-      img, H, W, (bf16*)out_slot, Hp, Wp, Cp, mean3_host[0], mean3_host[1], mean3_host[2], std3_host[0],
-      std3_host[1], std3_host[2]);
-  return check_launch("preprocess");
-}
-extern "C" int32_t c3d_preprocess_image_u8(const uint8_t* img, int32_t H, int32_t W, void* out_slot, int32_t Hp,
-                                           int32_t Wp, int32_t Cp, const float* mean3_host, const float* std3_host,
-                                           void* stream) {
-  C3D_REQ(img && out_slot && mean3_host && std3_host && Cp % 8 == 0 && Hp >= H && Wp >= W, "preprocess: bad args");
-  preprocess_kernel<uint8_t><<<grid_for((long long)Hp * Wp, 256), 256, 0, (cudaStream_t)stream>>>(
-      img, H, W, (bf16*)out_slot, Hp, Wp, Cp, mean3_host[0], mean3_host[1], mean3_host[2], std3_host[0],
-      std3_host[1], std3_host[2]);
-  return check_launch("preprocess_u8");
-}
 extern "C" int32_t c3d_pack_conv_weights_batched(const void* descs_dev, int32_t n, int64_t total_elems, void* stream) {
   C3D_REQ(descs_dev && n > 0 && total_elems > 0, "pack_conv_weights_batched: bad args");
   pack_conv_weights_batched_kernel<<<grid_for(total_elems, 256), 256, 0, (cudaStream_t)stream>>>(
@@ -927,12 +869,16 @@ extern "C" int32_t c3d_zero_stuff2(const void* dy, void* z, int32_t N, int32_t H
   return check_launch("zero_stuff2");
 }
 
-extern "C" int32_t c3d_pack_conv_weight(const float* w_oihw, int32_t Cout, int32_t Cin, int32_t KH, int32_t KW,
-                                        int32_t src_is_ohwi, void* fwd_ohwi, void* dgrad_ihwo, void* stream) {
-  C3D_REQ(w_oihw && (fwd_ohwi || dgrad_ihwo), "pack_conv_weight: bad args");
-  long long total = (long long)Cout * Cin * KH * KW;
+extern "C" int32_t c3d_pack_conv_weight(const c3d_pack_desc* desc_host, void* stream) {
+  C3D_REQ(desc_host && desc_host->src, "pack_conv_weight: null source");
+  const c3d_pack_desc D = *desc_host;
+  const bool phases = D.phase[0] || D.phase[1] || D.phase[2] || D.phase[3];
+  C3D_REQ(D.fwd || D.dgrad || phases, "pack_conv_weight: no output");
+  C3D_REQ(!phases || (D.phase[0] && D.phase[1] && D.phase[2] && D.phase[3] && D.KH == 3 && D.KW == 3),
+          "pack_conv_weight: phase outputs need all four buffers and a 3x3 weight");
+  C3D_REQ(D.Cout >= 0 && D.Cin >= 0 && D.KH >= 0 && D.KW >= 0, "pack_conv_weight: negative size");
+  const long long total = (long long)D.Cout * D.Cin * D.KH * D.KW;
   if (total == 0) return C3D_OK;
-  pack_conv_weight_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(w_oihw, Cout, Cin, KH, KW, src_is_ohwi,
-                                                                                  (bf16*)fwd_ohwi, (bf16*)dgrad_ihwo);
+  pack_conv_weight_desc_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(D, total);
   return check_launch("pack_conv_weight");
 }

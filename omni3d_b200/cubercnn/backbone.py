@@ -41,7 +41,7 @@ def _folded(conv, bn, cin):
         w, b = folded_conv_params(conv.weight.detach(), bn)
         if w.shape[1] != cin:
             w = F.pad(w, (0, 0, 0, 0, 0, cin - w.shape[1]))
-        wp, _ = K.pack_conv_weight(w, want_dgrad=False)
+        wp = K.pack_conv_weight(w, want_dgrad=False)[0]
         hit = (ver, wp, b.contiguous(), bn)
         _fold_cache[id(bn)] = hit
     return hit[1], hit[2]

@@ -8,8 +8,6 @@ gt_boxes3D, gt_poses — cubercnn/data/dataset_mapper.py:133-155) or the plain `
 omni3d_b200.synth.  EventStorage scalars the reference logs with .item() syncs are kept as device tensors
 in `model.metrics` (one async read by the caller instead of ~20 host syncs per step).
 """
-import os
-
 import torch
 from torch import nn
 
@@ -120,29 +118,6 @@ class RCNN3D(nn.Module):
             st["gt"] = collate_gt(batched_inputs, dev)
         return st
 
-    def _prelabel_async(self, x, gt):
-        """RPN anchor labelling + sampling depends on the GT only: run its ~60 small launches on a side stream while
-        the backbone occupies the main one (fork/join; also valid inside a CUDA-graph capture).  Every tensor it
-        produces stays referenced until after the join, and the side stream allocates nothing outside this region."""
-        if not os.environ.get("C3D_SIDE_STREAM"):      # opt-in: the small launches contend with the persistent conv
-            return None                                # CTAs
-        pg = self.proposal_generator
-        Hp, Wp = int(x.shape[1]), int(x.shape[2])
-        shapes = []
-        for s in pg.strides:
-            top = self.backbone.size_divisibility
-            if s <= top:
-                shapes.append((Hp // s, Wp // s))
-            else:                                    # p6 = stride-2 subsample of the coarsest FPN level (ceil)
-                k = s // top
-                shapes.append((-(-(Hp // top) // k), -(-(Wp // top) // k)))
-        if getattr(self, "_side", None) is None:
-            self._side = torch.cuda.Stream(device=x.device)
-        cur = torch.cuda.current_stream()
-        self._side.wait_stream(cur)
-        with torch.cuda.stream(self._side):
-            return pg.prelabel(shapes, gt, x.device)
-
     def forward_staged(self, st, _inject=None, batched_inputs=None):
         x = self._normalize(st)
         sizes, meta = st["sizes"], st["meta"]
@@ -151,16 +126,13 @@ class RCNN3D(nn.Module):
             gt = dict(st["gt"])
             if _inject:
                 gt.update(_inject)
-            pre = self._prelabel_async(x, gt)
             features = self.backbone(x)
-            if pre is not None:
-                torch.cuda.current_stream().wait_stream(self._side)
             # every FPN map feeds the RPN head AND the RoI pooler: one alias per consumer, so the RPN conv's data gradient
             # is added into the pooler's gradient inside the conv epilogue (nnfunc.fork) instead of by an add pass
             f_rpn, f_roi = {}, {}
             for k, v in features.items():
                 f_rpn[k], f_roi[k] = fork(v, 2)
-            proposals, l_rpn = self.proposal_generator(f_rpn, sizes, gt, sizes_dev=hw, prelabel=pre)
+            proposals, l_rpn = self.proposal_generator(f_rpn, sizes, gt, sizes_dev=hw)
             _, losses = self.roi_heads(f_roi, proposals, sizes, Ks, ratios, gt, im_h=hw[:, 0], meta=meta)
             losses.update(l_rpn)
             self.metrics = {**self.proposal_generator.stats, **self.roi_heads.stats}

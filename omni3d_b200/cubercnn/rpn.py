@@ -372,14 +372,7 @@ class RPNWithIgnore(nn.Module):
         out_s = torch.where(pad, torch.full_like(out_s, -float("inf")), out_s)
         return out_b, out_s, kcnt
 
-    def prelabel(self, shapes, gt, device):
-        """anchor labels + matches need only the GT and the feature-map shapes: callable before the features exist."""
-        if gt.get("anchor_labels") is not None:
-            return None
-        anchors = torch.cat(self.anchor_generator(list(shapes), device), 0)
-        return tuple(shapes), self.label_and_sample_anchors(anchors, gt["boxes"], gt["classes"], gt["present"])
-
-    def forward(self, features, image_sizes, gt=None, sizes_dev=None, prelabel=None):
+    def forward(self, features, image_sizes, gt=None, sizes_dev=None):
         feats = [features[f] for f in self.in_features]
         shapes = [tuple(f.shape[1:3]) for f in feats]
         anchors_l = self.anchor_generator(shapes, feats[0].device)
@@ -392,8 +385,6 @@ class RPNWithIgnore(nn.Module):
                 labels = gt["anchor_labels"]
                 valid = gt["present"] & (gt["classes"] >= 0)
                 idx = self.match_anchors(anchors, gt["boxes"], valid)[0]
-            elif prelabel is not None and prelabel[0] == tuple(shapes):
-                labels, idx = prelabel[1]                      # computed on a side stream during the backbone forward
             else:
                 labels, idx = self.label_and_sample_anchors(anchors, gt["boxes"], gt["classes"], gt["present"])
             losses = self.losses(anchors, logits, deltas, labels, idx, gt["boxes"])

@@ -127,21 +127,21 @@ def preprocess_images(images, mean, std, size_divisibility=64, cpad=16):
     out = torch.empty((len(images), Hp, Wp, cpad), device=images[0].device, dtype=torch.bfloat16)
     m = (f32 * 3)(*[float(v) for v in mean])
     s = (f32 * 3)(*[float(v) for v in std])
-    dt = images[0].dtype
-    if all(im.dtype == dt for im in images):            # the usual case: one launch for the whole batch
-        n = len(images)
-        for im in images:
-            assert im.dtype in (torch.float32, torch.uint8) and im.is_contiguous() and im.is_cuda
-        ptrs = (vp * n)(*[im.data_ptr() for im in images])
-        hs = (i32 * n)(*[im.shape[1] for im in images])
-        ws = (i32 * n)(*[im.shape[2] for im in images])
-        _lib.check(L.c3d_preprocess_batch(ptrs, hs, ws, n, int(dt == torch.uint8), ptr(out), Hp, Wp, cpad, m, s, stream()),
-                   launches=(n + 63) // 64)
-        return out
-    for i, im in enumerate(images):
+    for im in images:
         assert im.dtype in (torch.float32, torch.uint8) and im.is_contiguous() and im.is_cuda
-        fn = L.c3d_preprocess_image if im.dtype == torch.float32 else L.c3d_preprocess_image_u8
-        _lib.check(fn(ptr(im), im.shape[1], im.shape[2], ptr(out[i]), Hp, Wp, cpad, m, s, stream()))
+
+    def run(ims, dst):
+        n = len(ims)
+        ptrs = (vp * n)(*[im.data_ptr() for im in ims])
+        hs = (i32 * n)(*[im.shape[1] for im in ims])
+        ws = (i32 * n)(*[im.shape[2] for im in ims])
+        _lib.check(L.c3d_preprocess_batch(ptrs, hs, ws, n, int(ims[0].dtype == torch.uint8), ptr(dst), Hp, Wp, cpad, m, s,
+                                          stream()), launches=(n + 63) // 64)
+    if all(im.dtype == images[0].dtype for im in images):     # the usual case: one launch for the whole batch
+        run(images, out)
+    else:                                                    # uint8 and fp32 images mixed: one launch per image
+        for i, im in enumerate(images):
+            run([im], out[i])
     return out
 
 

@@ -6,7 +6,6 @@ kernels' bf16 OHWI layouts once per parameter version.  Forward AND backward run
   conv fwd  -> c3d_conv2d_fwd          dgrad -> c3d_conv2d_fwd with flipped/transposed weights
   wgrad     -> c3d_conv2d_wgrad        BN    -> c3d_bn_finalize / c3d_bn_apply / c3d_bn_bwd
 """
-import os
 import weakref
 
 import torch
@@ -15,7 +14,9 @@ from . import _lib
 from . import conv as K
 from . import kernels as Kx
 
-_pack_cache = {}
+# bf16 kernel-layout packs of the fp32 masters, per nn.Parameter: {id: ((version key), weak reference, packs)}
+_pack_cache = {}        # conv weights: (fwd, dgrad, stride-2 phase packs or None)
+_lin_cache = {}         # linear weights: (chw, fwd, transposed)
 _epoch = 0
 
 
@@ -25,7 +26,6 @@ def invalidate_packed():
     global _epoch
     _epoch += 1
     _pack_cache.clear()
-    _phase_cache.clear()
     _lin_cache.clear()
 
 
@@ -39,22 +39,28 @@ def _cache_key(w):
     return id(w), (w.data_ptr(), w._version, _epoch, tuple(w.shape), tuple(w.stride()))
 
 
-def _packed(w, kind):
-    """bf16 kernel-layout copies of an fp32 OIHW master — (Cout,KH,KW,Cin) for the forward pass and
-    (Cin,KH,KW,Cout) with the taps rotated by 180 degrees for the data gradient — produced by ONE
-    c3d_pack_conv_weight launch and cached per (parameter object, storage, version, optimizer epoch)."""
+def _cache_get(cache, w):
+    """the packs cached for parameter w, or None when there are none or they are stale"""
     key, ver = _cache_key(w)
-    hit = _pack_cache.get(key) if key is not None else None
-    if hit is None or hit[0] != ver or hit[3]() is not w:
-        f, g = K.pack_conv_weight(w)
-        hit = (ver, f, g, weakref.ref(w) if key is not None else None)
-        if key is not None:
-            _pack_cache[key] = hit
-    return hit[1] if kind == "fwd" else hit[2]
+    hit = cache.get(key) if key is not None else None
+    return hit[2] if hit is not None and hit[0] == ver and hit[1]() is w else None
 
 
-_phase_cache = {}
-_tap_index = {}
+def _cache_put(cache, w, packs):
+    key, ver = _cache_key(w)
+    if key is not None:
+        cache[key] = (ver, weakref.ref(w), packs)
+    return packs
+
+
+def _packed(w, phases=False):
+    """(fwd, dgrad, phase packs) of an fp32 OIHW / channels_last conv master (conv.pack_desc) — the phase sub-kernels of a
+    3x3 stride-2 data gradient only when asked for (else None) — produced by ONE pack launch and cached per parameter."""
+    hit = _cache_get(_pack_cache, w)
+    if hit is None or (phases and hit[2] is None):
+        hit = _cache_put(_pack_cache, w, K.pack_conv_weight(w, phases=_phase_layout(w) if phases else None))
+    return hit
+
 
 # ---- all conv weights of a model packed by ONE launch per step (c3d_pack_conv_weights_batched) ----------------------------
 _plans = {}
@@ -62,9 +68,9 @@ _plans = {}
 
 def prepack_model(model):
     """Pack every directly-used conv weight of `model` (forward OHWI pack, rotated data-gradient pack, and the four phase
-    sub-kernels of 3x3 / stride-2 layers) with one kernel launch and seed the per-parameter caches, so the layer-by-layer
-    `_packed` / `_phase_packs` look-ups of this step are hits.  Output buffers and the descriptor table are built once per
-    model (stable addresses: CUDA-graph safe); call at the start of every training step, after the optimizer update."""
+    sub-kernels of 3x3 / stride-2 layers) with one kernel launch and seed the per-parameter cache, so the layer-by-layer
+    `_packed` look-ups of this step are hits.  Output buffers and the descriptor table are built once per model (stable
+    addresses: CUDA-graph safe); call at the start of every training step, after the optimizer update."""
     convs = [m for m in model.modules() if isinstance(m, torch.nn.Conv2d) and isinstance(m.weight, torch.nn.Parameter)
              and m.weight.is_cuda and m.weight.shape[1] % 16 == 0 and m.weight.shape[0] % 16 == 0]
     if not convs:
@@ -72,45 +78,25 @@ def prepack_model(model):
     key = tuple((id(m.weight), m.weight.data_ptr(), tuple(m.weight.stride())) for m in convs)
     plan = _plans.get(id(model))
     if plan is None or plan["key"] != key:
-        dev = convs[0].weight.device
         arr = (_lib.PackDesc * len(convs))()
         bufs, start = [], 0
         for i, m in enumerate(convs):
             w = m.weight
             O, I, KH, KW = w.shape
-            ohwi = (not w.is_contiguous()) and w.permute(0, 2, 3, 1).is_contiguous()
-            if not (ohwi or w.is_contiguous()):
-                raise RuntimeError("prepack_model: conv weight storage is neither OIHW nor OHWI")
-            phase = m.stride[0] == 2 and KH == 3 and KW == 3 and m.padding[0] == 1
-            f = torch.empty((O, KH, KW, I), device=dev, dtype=torch.bfloat16)
-            g = torch.empty((I, KH, KW, O), device=dev, dtype=torch.bfloat16)
-            merged = phase and _merge_phases(I, O)
-            if merged:          # ONE (4*I, 2, 2, O) weight: row block (a,b) = phase (a,b); unused taps stay zero for ever
-                mg = torch.zeros((4 * I, 2, 2, O), device=dev, dtype=torch.bfloat16)
-                ph = {"merged": mg, **{(a, b): mg[(2 * a + b) * I:(2 * a + b + 1) * I] for a in (0, 1) for b in (0, 1)}}
-            else:
-                ph = {(a, b): torch.empty((I, 2 if a else 1, 2 if b else 1, O), device=dev, dtype=torch.bfloat16)
-                      for a in (0, 1) for b in (0, 1)} if phase else None
-            d = arr[i]
-            d.src, d.fwd, d.dgrad = w.data_ptr(), f.data_ptr(), g.data_ptr()
-            for a in (0, 1):
-                for b in (0, 1):
-                    d.phase[a * 2 + b] = ph[(a, b)].data_ptr() if ph else None
-            d.start, d.Cout, d.Cin, d.KH, d.KW, d.src_is_ohwi, d.merged_phases = start, O, I, KH, KW, int(ohwi), int(bool(merged))
+            phases = m.stride[0] == 2 and KH == 3 and KW == 3 and m.padding[0] == 1
+            arr[i], packs = K.pack_desc(w, phases=_phase_layout(w) if phases else None)
+            arr[i].start = start
             start += w.numel()
-            bufs.append((w, f, g, ph))
-        table = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
+            bufs.append((w, packs))
+        table = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(convs[0].weight.device)
         plan = _plans[id(model)] = {"key": key, "table": table, "bufs": bufs, "total": start, "n": len(convs)}
     _lib.check(_lib.lib().c3d_pack_conv_weights_batched(plan["table"].data_ptr(), plan["n"], plan["total"], _lib.stream()))
-    for w, f, g, ph in plan["bufs"]:
-        k, ver = _cache_key(w)
-        _pack_cache[k] = (ver, f, g, weakref.ref(w))
-        if ph is not None:
-            _phase_cache[k] = (ver, ph, weakref.ref(w))
+    for w, packs in plan["bufs"]:
+        _cache_put(_pack_cache, w, packs)
     return plan["n"]
 
 
-_MERGE_MAX_O = int(os.environ.get("C3D_DGRAD_MERGE_MAX_O", "256"))
+_MERGE_MAX_O = 256
 
 
 def _merge_phases(I, O):
@@ -120,37 +106,8 @@ def _merge_phases(I, O):
     return O <= _MERGE_MAX_O and (2 * I) % 16 == 0 and O % 16 == 0
 
 
-def _phase_packs(w):
-    """sub-kernels of a 3x3 / stride-2 / pad-1 conv's data gradient, one per output parity (a,b):
-    dx[2i+a, 2j+b] = sum_{k'} dy[i+k'h, j+k'w] * W[.., kh(a,k'h), kw(b,k'w)] with kh(0,.) = [1], kh(1,.) = [2,0].
-    -> {(a,b): bf16 (Cin, KH', KW', Cout)}, cached per parameter version / optimizer epoch."""
-    key, ver = _cache_key(w)
-    hit = _phase_cache.get(key) if key is not None else None
-    if hit is not None and hit[0] == ver and hit[2]() is w:
-        return hit[1]
-    taps = _tap_index.get(w.device)
-    if taps is None:          # device-resident index tensors, built once (a python-list index is a host->device copy)
-        taps = _tap_index[w.device] = {0: torch.tensor([1], device=w.device), 1: torch.tensor([2, 0], device=w.device)}
-    packs = {}
-    O, I = w.shape[0], w.shape[1]
-    with torch.no_grad():
-        if _merge_phases(I, O):
-            mg = torch.zeros((4 * I, 2, 2, O), device=w.device, dtype=torch.bfloat16)
-            for a in (0, 1):
-                for b in (0, 1):
-                    sub = w.index_select(2, taps[a]).index_select(3, taps[b])   # (Cout,Cin,KH',KW')
-                    blk = mg[(2 * a + b) * I:(2 * a + b + 1) * I]
-                    blk[:, :sub.shape[2], :sub.shape[3], :] = sub.permute(1, 2, 3, 0).to(torch.bfloat16)
-                    packs[(a, b)] = blk
-            packs["merged"] = mg
-        else:
-            for a in (0, 1):
-                for b in (0, 1):
-                    sub = w.index_select(2, taps[a]).index_select(3, taps[b])   # (Cout,Cin,KH',KW')
-                    packs[(a, b)] = sub.permute(1, 2, 3, 0).contiguous().to(torch.bfloat16)
-    if key is not None:
-        _phase_cache[key] = (ver, packs, weakref.ref(w))
-    return packs
+def _phase_layout(w):
+    return "merged" if _merge_phases(w.shape[1], w.shape[0]) else "separate"
 
 
 def _dgrad(dy, w, stride, pad, in_hw, into=None):
@@ -164,7 +121,7 @@ def _dgrad(dy, w, stride, pad, in_hw, into=None):
         N, Ho, Wo, _ = dy.shape
         H, W = in_hw
         dx = into if acc else torch.empty((N, H, W, w.shape[1]), device=dy.device, dtype=dy.dtype)
-        packs = _phase_packs(w)
+        packs = _packed(w, phases=True)[2]
         I = w.shape[1]
         if "merged" in packs and dx.stride(2) == I:
             # channel j = (a, b, ci) of dy-pixel (h, w) is dx[2h + a, 2w + b, ci]: in a DENSE dx (b, ci) are 2*I contiguous
@@ -181,7 +138,7 @@ def _dgrad(dy, w, stride, pad, in_hw, into=None):
             K.conv2d_fwd(dy, wp, stride=1, pad=0, out=dx, out_place=(H * W, 2 * W, 2, a * W + b), out_hw_override=(Ho, Wo),
                          accumulate=acc)
         return dx
-    wp = _packed(w, "dgrad")
+    wp = _packed(w)[1]
     if stride == 1:
         return K.conv2d_fwd(dy, wp, stride=1, pad=KH - 1 - pad, out=into, accumulate=acc)
     assert stride == 2
@@ -232,7 +189,7 @@ def _grad_slot(p):
 # returns None.  _Fork.backward — which autograd runs after all consumers — folds in whatever reached it as a plain
 # tensor (consumers that know nothing of sinks) and hands the buffer to the producer.  Same sums as autograd's, with
 # the adds done in fp32 before the single bf16 rounding.
-GRAD_CHAIN = os.environ.get("C3D_NO_GRAD_CHAIN") is None
+GRAD_CHAIN = True      # False: plain autograd sums (the reference the gradient-chaining tests compare against)
 
 
 class _GradSink:
@@ -336,7 +293,7 @@ class ConvBNAct(torch.autograd.Function):
     def forward(ctx, x, w, gamma, beta, running_mean, running_var, residual, stride, pad, relu, training, eps,
                 momentum):
         x = x.contiguous()
-        wp = _packed(w, "fwd")
+        wp = _packed(w)[0]
         if training:
             y, stats = K.conv2d_fwd(x, wp, stride=stride, pad=pad, want_stats=True)
             count = y.numel() // y.shape[-1]
@@ -379,7 +336,7 @@ class ConvBias(torch.autograd.Function):
     def forward(ctx, x, w, bias, addend, stride, pad, relu, out_fp32):
         x = x.contiguous()
         add = addend.contiguous() if addend is not None else None
-        out = K.conv2d_fwd(x, _packed(w, "fwd"), bias, stride, pad, relu=relu, addend=add, up2=add is not None,
+        out = K.conv2d_fwd(x, _packed(w)[0], bias, stride, pad, relu=relu, addend=add, up2=add is not None,
                            out_fp32=out_fp32)
         ctx.save_for_backward(x, w, out if relu else None, bias)
         ctx.cfg = (stride, pad, relu, addend is not None, bias is not None)
@@ -399,18 +356,11 @@ class ConvBias(torch.autograd.Function):
         return dx, dw, dbias if ret_b else None, dadd, None, None, None, None
 
 
-_lin_cache = {}
-
-
 def _packed_linear(w, chw):
     """bf16 (N,K') forward operand and its (K',N) transpose for the data gradient, cached like the conv packs."""
-    key, ver = _cache_key(w)
-    hit = _lin_cache.get(key) if key is not None else None
-    if hit is None or hit[0] != (ver, chw) or hit[3]() is not w:
-        f, t = K.pack_linear_weight(w, chw)
-        hit = ((ver, chw), f, t, weakref.ref(w) if key is not None else None)
-        if key is not None:
-            _lin_cache[key] = hit
+    hit = _cache_get(_lin_cache, w)
+    if hit is None or hit[0] != chw:
+        hit = _cache_put(_lin_cache, w, (chw,) + K.pack_linear_weight(w, chw))
     return hit[1], hit[2]
 
 

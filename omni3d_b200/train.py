@@ -11,7 +11,6 @@ cubercnn/solver/build.py:6-69 (build_optimizer), re-designed for one-process-per
   memory one step late (no per-step synchronisation, vs 3 barriers + 3 scalar all-reduces + ~10 .item()).
 """
 import math
-import os
 
 import torch
 import torch.distributed as dist
@@ -55,7 +54,7 @@ def lr_at(cfg, it):
 
 
 class FlatSGDTrainer:
-    def __init__(self, cfg, model, channels_last_weights=True, use_graph=None):
+    def __init__(self, cfg, model, channels_last_weights=True, use_graph=True, split_backward=False):
         if cfg.SOLVER.TYPE != "sgd":
             raise ValueError("{} is not supported as an optimizer on the accelerated path.".format(cfg.SOLVER.TYPE))
         if getattr(cfg.SOLVER, "NESTEROV", False):
@@ -150,30 +149,26 @@ class FlatSGDTrainer:
         self.iteration = 0
         self.steps_run = 0                      # steps executed by THIS object (graph warm-up; `iteration` may be restored)
         self.stabilize = cfg.MODEL.STABILIZE > 0
-        # CUDA-graph replay of the step body (see step() / _body()); C3D_TRAIN_GRAPH=0 disables it
-        if use_graph is None:
-            use_graph = os.environ.get("C3D_TRAIN_GRAPH") != "0"
+        # CUDA-graph replay of the step body (see step() / _body())
         self.use_graph = bool(use_graph) and self.on_cuda and hasattr(model, "forward_staged")
         self.graph_warmup = 2
         self.graph = self.static = self.graph_sig = self.graph_losses = self.graph_vec = None
         self.graph_launches = 0
         self.recaptures = 0
         self.lr_dev = torch.zeros(1, device=dev)
-        # two-stage backward (gradient all-reduce of the early bucket overlapped with the backbone's backward): several ranks,
-        # or forced for tests; the model cuts its autograd graph at the bottom-up outputs when told to
-        self.split_backward = bool(late) and hasattr(model, "set_backward_cut") and \
-            (self.world > 1 or bool(os.environ.get("C3D_TRAIN_SPLIT_BACKWARD")))
+        # two-stage backward (gradient all-reduce of the early bucket overlapped with the backbone's backward): always on several
+        # ranks, on one rank when split_backward asks for it; the model cuts its autograd graph at the bottom-up outputs when told to
+        self.split_backward = bool(late) and hasattr(model, "set_backward_cut") and (self.world > 1 or split_backward)
         if hasattr(model, "set_backward_cut"):
             model.set_backward_cut(self.split_backward)
         self._pending = self._works = self._graph_split = None
-        self.prepack = os.environ.get("C3D_NO_PREPACK") is None and hasattr(model, "forward_staged")
 
     # -------------------------------------------------------------------------------------------------
     def _seg_forward(self, staged):
         """segment A: zero the gradient arena, forward, the 10 local losses as one vector."""
         model = self.model
         self.flat_g.zero_()
-        if self.on_cuda and self.prepack:
+        if self.on_cuda and hasattr(model, "forward_staged"):
             nnfunc.prepack_model(model)          # every conv weight's bf16 packs in one launch (instead of ~60 + ~70 ATen)
         loss_dict = model.forward_staged(staged) if hasattr(model, "forward_staged") else model(staged)
         vec = torch.stack([loss_dict[k].detach().float() if k in loss_dict else self.flat_g.new_zeros(())
@@ -377,9 +372,6 @@ class FlatSGDTrainer:
             return losses
         except Exception as e:      # noqa: BLE001 — never silently: say so, then keep training eagerly
             import sys
-            import traceback
-            if os.environ.get("C3D_DEBUG"):
-                traceback.print_exc()
             print("omni3d_b200: CUDA graph capture of the train step failed (%s: %s); continuing eagerly"
                   % (type(e).__name__, e), file=sys.stderr)
             self.use_graph, self.graph, self.static = False, None, None

@@ -163,6 +163,13 @@ def test_host_side_entry_points_without_gpu():
     assert rc != 0 and b"anchor_match" in L.c3d_last_error()
     with pytest.raises(_lib.C3DError):
         _lib.check(rc)
+    # c3d_pack_conv_weight: null source, no output, stride-2 phase outputs for a weight that is not 3x3
+    p = [ctypes.c_void_p(256 * k) for k in range(1, 8)]   # non-null dummies: every case is rejected before they are used
+    pack = lambda **kw: L.c3d_pack_conv_weight(ctypes.byref(_lib.PackDesc(**{**dict(Cout=16, Cin=16, KH=3, KW=3), **kw})), None)
+    assert pack(fwd=p[1], dgrad=p[2]) == _lib.C3D_EINVAL and b"null source" in L.c3d_last_error()
+    assert pack(src=p[0]) == _lib.C3D_EINVAL and b"no output" in L.c3d_last_error()
+    assert pack(src=p[0], fwd=p[1], phase=(ctypes.c_void_p * 4)(*p[3:7]), KH=1, KW=1) == _lib.C3D_EINVAL \
+        and b"3x3" in L.c3d_last_error()
 
 
 def test_conv_descriptor_argument_checks_without_gpu():

@@ -156,38 +156,76 @@ def test_bn_backward_mask_recomputed_from_y_equals_mask_from_out(C, frozen):
         assert torch.equal(a, b)
 
 
-def test_prepack_model_equals_per_parameter_packs():
-    """c3d_pack_conv_weights_batched (one launch for every conv weight: forward, data-gradient and stride-2 phase packs)
-    == the per-parameter pack kernel / torch formulation it replaces, for OIHW and channels-last (trainer arena) masters."""
+def _ref_conv_packs(w, phases):
+    """torch formulation of the bf16 conv-weight packs: forward (Cout,KH,KW,Cin), data gradient (Cin,KH,KW,Cout) rotated by
+    180 degrees, and the stride-2 phase sub-kernels {(a, b): (Cin,KH',KW',Cout)} with parity 0 -> tap [1], parity 1 -> taps
+    [2, 0]; "merged": the four phases as 2x2 row blocks of one zero-initialised (4*Cin,2,2,Cout) weight."""
+    w = w.detach()
+    O, I = w.shape[:2]
+    ref = {"fwd": w.permute(0, 2, 3, 1).bfloat16(), "dgrad": w.flip(2, 3).permute(1, 2, 3, 0).bfloat16()}
+    if phases is None:
+        return ref
+    taps = {0: [1], 1: [2, 0]}
+    mg = torch.zeros((4 * I, 2, 2, O), device=w.device, dtype=torch.bfloat16)
+    for a in (0, 1):
+        for b in (0, 1):
+            sub = w[:, :, taps[a]][:, :, :, taps[b]].permute(1, 2, 3, 0).bfloat16()
+            if phases == "merged":
+                blk = mg[(2 * a + b) * I:(2 * a + b + 1) * I]
+                blk[:, :sub.shape[1], :sub.shape[2]] = sub
+                sub = blk
+            ref[(a, b)] = sub
+    if phases == "merged":
+        ref["merged"] = mg
+    return ref
+
+
+def _check_conv_packs(packs, w, phases):
+    f, g, ph = packs
+    ref = _ref_conv_packs(w, phases)
+    assert torch.equal(f, ref.pop("fwd")) and torch.equal(g, ref.pop("dgrad"))
+    if phases is None:
+        assert ph is None
+        return
+    assert ph.keys() == ref.keys()
+    for k in ref:
+        assert torch.equal(ph[k], ref[k]), k
+
+
+def test_conv_weight_packs_equal_torch_reference():
+    """c3d_pack_conv_weights_batched (one launch for every conv weight of a model) and c3d_pack_conv_weight (one weight)
+    == the torch formulation of the forward, data-gradient and stride-2 phase packs, for OIHW and channels-last (trainer
+    arena) masters, merged and separate phase layouts; a parameter update invalidates the cached packs."""
     from omni3d_b200 import conv as K
     from omni3d_b200 import nnfunc
 
     class Net(torch.nn.Module):
         def __init__(self):
             super().__init__()
-            self.a = torch.nn.Conv2d(16, 32, 3, stride=2, padding=1, bias=False)
+            self.a = torch.nn.Conv2d(16, 32, 3, stride=2, padding=1, bias=False)      # merged phases
             self.b = torch.nn.Conv2d(32, 64, 3, padding=1, bias=False)
             self.c = torch.nn.Conv2d(64, 16, 1, bias=False)
+            self.d = torch.nn.Conv2d(32, 272, 3, stride=2, padding=1, bias=False)     # Cout > 256: separate phases
             self.skip = torch.nn.Conv2d(3, 16, 7, padding=3, bias=False)         # Cin 3: not packed here
     net = Net().cuda()
     with torch.no_grad():                          # channels-last storage like the trainer's arena
-        w = net.b.weight
-        net.b.weight.data = w.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
-    assert nnfunc.prepack_model(net) == 3
-    for m in (net.a, net.b, net.c):
-        f, g = K.pack_conv_weight(m.weight)
-        assert torch.equal(nnfunc._packed(m.weight, "fwd"), f) and torch.equal(nnfunc._packed(m.weight, "dgrad"), g)
-    ref = {}
-    nnfunc._phase_cache.clear()
-    got = None
-    nnfunc.prepack_model(net)
-    got = {k: v.clone() for k, v in nnfunc._phase_packs(net.a.weight).items()}
-    nnfunc._phase_cache.clear()
-    ref = nnfunc._phase_packs(net.a.weight)                       # torch formulation (cache was cleared)
-    for k in ref:
-        assert torch.equal(got[k], ref[k]), k
-    # a parameter update (version bump) invalidates the seeded entries
+        for m in (net.b, net.d):
+            m.weight.data = m.weight.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
+    layers = {net.a: "merged", net.b: None, net.c: None, net.d: "separate"}
+    assert nnfunc._phase_layout(net.a.weight) == "merged" and nnfunc._phase_layout(net.d.weight) == "separate"
+    nnfunc.invalidate_packed()
+    assert nnfunc.prepack_model(net) == 4
+    for m, phases in layers.items():
+        _check_conv_packs(nnfunc._packed(m.weight), m.weight, phases)                    # seeded by prepack_model
+        for layout in ("merged", "separate", None) if m.kernel_size == (3, 3) else (None,):         # one weight, one launch
+            _check_conv_packs(K.pack_conv_weight(m.weight, phases=layout), m.weight, layout)
+    f, _, _ = K.pack_conv_weight(net.b.weight, want_dgrad=False)
+    assert torch.equal(f, _ref_conv_packs(net.b.weight, None)["fwd"])
+    # a parameter update (version bump) invalidates the seeded entries; the repack of a cached entry without phases adds them
     with torch.no_grad():
         net.c.weight.add_(1.0)
-    f2, _ = K.pack_conv_weight(net.c.weight)
-    assert torch.equal(nnfunc._packed(net.c.weight, "fwd"), f2)
+        net.a.weight.mul_(-0.5)
+    _check_conv_packs(nnfunc._packed(net.c.weight), net.c.weight, None)
+    _check_conv_packs(nnfunc._packed(net.a.weight), net.a.weight, None)
+    _check_conv_packs(nnfunc._packed(net.a.weight, phases=True), net.a.weight, "merged")
+    nnfunc.invalidate_packed()

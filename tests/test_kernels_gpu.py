@@ -127,15 +127,17 @@ def test_preprocess_matches_reference_formula():
     from omni3d_b200 import kernels as Kx
     imgs = [torch.randint(0, 256, (3, 50, 70), device="cuda").float(), torch.randint(0, 256, (3, 64, 40), device="cuda").float()]
     mean, std = [103.53, 116.28, 123.675], [57.375, 57.12, 58.395]
-    out = Kx.preprocess_images(imgs, mean, std, 64, 16)
-    assert tuple(out.shape) == (2, 64, 128, 16)
     m, s = torch.tensor(mean, device="cuda").view(3, 1, 1), torch.tensor(std, device="cuda").view(3, 1, 1)
-    for i, im in enumerate(imgs):
-        ref = ((im - m) / s).bfloat16().float()
-        got = out[i, :im.shape[1], :im.shape[2], :3].float().permute(2, 0, 1)
-        assert torch.equal(got, ref)
-        assert out[i, im.shape[1]:].abs().sum() == 0 and out[i, :, im.shape[2]:].abs().sum() == 0
-        assert out[i, ..., 3:].abs().sum() == 0
+    mixed = [imgs[0].to(torch.uint8), imgs[1], torch.randint(0, 256, (3, 33, 90), device="cuda", dtype=torch.uint8)]
+    for batch, shape in ((imgs, (2, 64, 128, 16)), (mixed, (3, 64, 128, 16))):      # one dtype, then uint8 and fp32 mixed
+        out = Kx.preprocess_images(batch, mean, std, 64, 16)
+        assert tuple(out.shape) == shape
+        for i, im in enumerate(batch):
+            ref = ((im.float() - m) / s).bfloat16().float()
+            got = out[i, :im.shape[1], :im.shape[2], :3].float().permute(2, 0, 1)
+            assert torch.equal(got, ref)
+            assert out[i, im.shape[1]:].abs().sum() == 0 and out[i, :, im.shape[2]:].abs().sum() == 0
+            assert out[i, ..., 3:].abs().sum() == 0
 
 
 def test_roi_align_fwd_bwd_vs_torchvision():

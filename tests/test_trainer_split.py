@@ -51,13 +51,9 @@ def _run(world_rank=None):
     cfg.SOLVER.BASE_LR, cfg.SOLVER.WARMUP_ITERS = 0.05, 0
     out = []
     for split in (False, True):
-        if split:
-            os.environ["C3D_TRAIN_SPLIT_BACKWARD"] = "1"
-        else:
-            os.environ.pop("C3D_TRAIN_SPLIT_BACKWARD", None)
         torch.manual_seed(0)
         m = ToyCut()
-        tr = FlatSGDTrainer(cfg, m)
+        tr = FlatSGDTrainer(cfg, m, split_backward=split)
         if dist.is_initialized() and dist.get_world_size() > 1:
             assert tr.split_backward            # several ranks: always on
         else:
@@ -69,11 +65,10 @@ def _run(world_rank=None):
         for _ in range(3):
             tr.step(x)
         out.append(tr.flat_p.clone())
-    os.environ.pop("C3D_TRAIN_SPLIT_BACKWARD", None)
     return out
 
 
-def test_split_backward_equals_single_backward_one_rank():
+def test_split_backward_argument_equals_single_backward_one_rank():
     a, b = _run()
     assert torch.allclose(a, b, atol=1e-7) and a.abs().sum() > 0
 
