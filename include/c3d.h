@@ -8,9 +8,10 @@
  *   - plain pointers + sizes; every pointer is DEVICE memory unless the name ends in _host;
  *   - the caller owns every buffer including the workspace (size from the matching
  *     *_workspace_bytes query); kernels never allocate, free or synchronise.  The one exception are the weight
- *     gradients (conv / linear wgrad) split over several CTAs: their per-split partial sums live in scratch from the
- *     stream-ordered allocator (cudaMallocAsync / cudaFreeAsync on `stream`, which graph capture records) and are
- *     added in split order, so the gradient is the same on every run;
+ *     gradients (conv / linear wgrad) split over several CTAs and the ROIAlign backward: the per-split partial sums
+ *     and the RoI buckets live in scratch from the stream-ordered allocator (cudaMallocAsync / cudaFreeAsync on
+ *     `stream`, which graph capture records), and the partial sums are added in split order, so the gradient is the
+ *     same on every run;
  *   - work is enqueued on `stream` (a cudaStream_t / CUstream handle passed as void*);
  *   - return 0 (C3D_OK) or a negative c3d_status; c3d_last_error() gives a thread-local string.
  */
@@ -261,7 +262,7 @@ int32_t c3d_sgd_momentum_dev(float* p, const float* g, float* mom, int64_t n, co
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
   const void* feat[5];   /* level l: bf16 (N,H[l],W[l],C) */
-  void* grad[5];         /* backward only: fp32 (N,H[l],W[l],C), += (each element in one fixed order) */
+  void* grad[5];         /* backward only: fp32 (N,H[l],W[l],C), written (every element, in one fixed order) */
   int32_t H[5], W[5];
   float scale[5];
   int32_t num_levels;

@@ -169,10 +169,10 @@ def roi_align_fwd(feats, strides, rois, pooled=7):
 
 
 def roi_align_bwd(feats, strides, rois, dout, pooled=7):
-    """-> list of fp32 gradient maps shaped like feats."""
+    """-> list of fp32 gradient maps shaped like feats (the kernel writes every element)."""
     L = _lib.lib()
     C = feats[0].shape[-1]
-    grads = [torch.zeros(f.shape, device=f.device, dtype=torch.float32) for f in feats]
+    grads = [torch.empty(f.shape, device=f.device, dtype=torch.float32) for f in feats]
     lv = _levels(feats, strides, grads)
     _lib.check(L.c3d_roi_align_bwd(ctypes.byref(lv), ptr(rois), rois.shape[0], C, pooled, pooled, ptr(dout), stream()))
     return grads
