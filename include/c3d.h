@@ -85,14 +85,14 @@ int32_t c3d_box3d_overlap_segmented(const float* boxes_dt, int64_t n_dt, const f
  * flipped/transposed weights; weight-gradient = c3d_conv2d_wgrad.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
-  int32_t N, H, W, Cin;      /* input  (N,H,W,Cin)  bf16, pixel stride x_pix_stride elements (0 => Cin) */
+  int32_t N, H, W, Cin;      /* input  (N,H,W,Cin)  bf16 */
   int32_t Cout, KH, KW;      /* weight (Cout,KH,KW,Cin) bf16 contiguous */
   int32_t stride, pad;       /* stride 1 or 2 (same in h and w), symmetric zero padding */
   int32_t relu;              /* epilogue: max(.,0) after bias/addend */
   int32_t out_fp32;          /* output fp32 instead of bf16 */
   int32_t add_mode;          /* 0 none; 1 addend (N,Ho,Wo,Cout); 2 addend (N,Ho/2,Wo/2,Cout) nearest-up x2 (FPN);
                                 3 accumulate in place: y (bf16) += result at the output's own (possibly strided) position */
-  int64_t x_pix_stride, y_pix_stride, add_pix_stride;   /* elements; 0 => dense */
+  int64_t y_pix_stride;      /* elements between output pixels; 0 => Cout */
   /* optional strided output placement (in pixels): y pixel index = n*y_img_stride + ho*y_h_stride + wo*y_w_stride +
    * y_offset; all 0 => dense (N,Ho,Wo).  Used by the phase-decomposed stride-2 data gradient. */
   int64_t y_img_stride, y_h_stride, y_w_stride, y_offset;
@@ -118,17 +118,14 @@ int32_t c3d_conv2d_tiles(const c3d_conv_desc* d, int32_t* tiles_m, int32_t* tile
 int32_t c3d_conv2d_fwd(const c3d_conv_desc* d, const void* x, const void* w, const float* bias,
                        const void* addend, void* y, float* stats, void* stream);
 
-/* dw[Cout][KH][KW][Cin] (fp32) += the weight gradient of the convolution described by d, from the
- * forward input x (N,H,W,Cin) and the output gradient dy (N,Ho,Wo,Cout), both bf16 NHWC.
- * Split-K over pixels, partials summed in a fixed order: the caller zeroes (or pre-loads) dw.
+/* dw (fp32) += the weight gradient of the convolution described by d, from the forward input x (N,H,W,Cin) and the
+ * output gradient dy (N,Ho,Wo,Cout), both bf16 NHWC.  dw is [Cout][KH][KW][Cin], or with oihw != 0 the fp32
+ * master-layout gradient [Cout][Cin][KH][KW] (accumulate straight into the optimizer's gradient arena, no layout
+ * conversion pass).  Split-K over pixels, partials summed in a fixed order: the caller zeroes (or pre-loads) dw.
  * Cin and Cout must be multiples of 16, except for the stride-1 thin-channel layers with (KH, Cin) in
  * {(7, 8), (3, 16), (3, 32)} and Cout 16 or 32 (same padding, W >= 128 unless Cin = 8), which run on the
  * rolling-halo kernel; other Cin = 8 layers return C3D_EINVAL. */
-int32_t c3d_conv2d_wgrad(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, void* stream);
-/* same, oihw != 0: dw is the fp32 master-layout gradient [Cout][Cin][KH][KW] (accumulate straight into the
- * optimizer's gradient arena, no layout conversion pass) */
-int32_t c3d_conv2d_wgrad_ex(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int32_t oihw,
-                            void* stream);
+int32_t c3d_conv2d_wgrad(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int32_t oihw, void* stream);
 /* Re-pack of one fp32 master conv weight src (Cout,Cin,KH,KW) — stored OIHW, or OHWI = torch channels_last storage when
  * src_is_ohwi != 0 — into any of these bf16 outputs (NULL = not written):
  *   fwd    (Cout,KH,KW,Cin) forward pack;
@@ -158,28 +155,25 @@ int32_t c3d_pack_conv_weights_batched(const void* descs_dev, int32_t n, int64_t 
  * (cubercnn/modeling/roi_heads/cube_head.py:63-73,108-144,146-197).
  *   x  (rows, K) bf16 row-major; w (N, K) bf16 = nn.Linear.weight; wt (K, N) bf16 = its transpose;
  *   K % 16 == 0, N % 16 == 0 (callers zero-pad the predictors).
- * c3d_pack_linear_weight: fp32 master (N, K) -> bf16 w (N, K') and (optional) wt (K', N).  C * PP == K with PP > 1
- *   re-orders the input features from (c, p) [NCHW-flattened RoI, the reference's layout] to (p, c) [NHWC-flattened RoI].
- * c3d_linear_wgrad: dw (fp32, +=) = dy^T x.  master_chw != 0: dw is addressed in the master's (c, p)
- *   feature order (accumulate straight into the optimizer's gradient arena), else in the packed (p, c) order.
+ * The rows = nseg * seg_rows feature vectors are nseg blocks of seg_rows consecutive rows that start every seg_stride rows
+ * inside a larger (.., K) matrix (x for fwd / wgrad, dx for dgrad); the other operand is dense.  A dense layer is
+ * nseg = 1, seg_stride = seg_rows = rows.  seg_rows <= INT32_MAX and seg_stride >= seg_rows, else C3D_EINVAL; nseg <= 0 or
+ * seg_rows <= 0 is an empty layer (C3D_OK, nothing launched).  The cube head reads the first Fc of every image's S pooled
+ * RoIs in place, and its data gradient is ACCUMULATED (accumulate != 0: dx += dy . W) into the box head's — no gather
+ * copy, no zero-padded scatter, no add pass.
+ * c3d_pack_linear_weight: fp32 master (N, K) -> bf16 w (N, K') and wt (K', N).  C * PP == K with PP > 1 re-orders the
+ *   input features from (c, p) [NCHW-flattened RoI, the reference's layout] to (p, c) [NHWC-flattened RoI].
+ * c3d_linear_wgrad: dw (fp32, +=) = dy^T x.  With PP > 1 dw is addressed in the master's (c, p) feature order (accumulate
+ *   straight into the optimizer's gradient arena).
  * ------------------------------------------------------------------------------------------ */
 int32_t c3d_pack_linear_weight(const float* w, int32_t N, int32_t K, int32_t C, int32_t PP, void* w_bf16, void* wt_bf16,
                                void* stream);
-int32_t c3d_linear_fwd(const void* x, const void* w, const float* bias, void* y, int64_t rows, int32_t K, int32_t N,
-                       int32_t relu, int32_t out_fp32, void* stream);
-int32_t c3d_linear_dgrad(const void* dy, const void* wt, void* dx, int64_t rows, int32_t N, int32_t K, void* stream);
-int32_t c3d_linear_wgrad(const void* x, const void* dy, float* dw, int64_t rows, int32_t K, int32_t N, int32_t C,
-                         int32_t PP, int32_t master_chw, void* stream);
-/* Row-block variants: the `rows` = nseg * seg_rows feature vectors are nseg blocks of seg_rows consecutive rows that start
- * every seg_stride rows inside a larger (.., K) matrix (x for fwd / wgrad, dx for dgrad); the other operand is dense.
- * The cube head reads the first Fc of every image's S pooled RoIs in place, and its data gradient is ACCUMULATED
- * (accumulate != 0: dx += dy . W) into the box head's — no gather copy, no zero-padded scatter, no add pass. */
-int32_t c3d_linear_fwd_blocks(const void* x, const void* w, const float* bias, void* y, int32_t nseg, int32_t seg_rows,
-                              int64_t seg_stride, int32_t K, int32_t N, int32_t relu, int32_t out_fp32, void* stream);
-int32_t c3d_linear_dgrad_blocks(const void* dy, const void* wt, void* dx, int32_t nseg, int32_t seg_rows, int64_t seg_stride,
-                                int32_t N, int32_t K, int32_t accumulate, void* stream);
-int32_t c3d_linear_wgrad_blocks(const void* x, const void* dy, float* dw, int32_t nseg, int32_t seg_rows, int64_t seg_stride,
-                                int32_t K, int32_t N, int32_t C, int32_t PP, int32_t master_chw, void* stream);
+int32_t c3d_linear_fwd(const void* x, const void* w, const float* bias, void* y, int32_t nseg, int64_t seg_rows,
+                       int64_t seg_stride, int32_t K, int32_t N, int32_t relu, int32_t out_fp32, void* stream);
+int32_t c3d_linear_dgrad(const void* dy, const void* wt, void* dx, int32_t nseg, int64_t seg_rows, int64_t seg_stride,
+                         int32_t N, int32_t K, int32_t accumulate, void* stream);
+int32_t c3d_linear_wgrad(const void* x, const void* dy, float* dw, int32_t nseg, int64_t seg_rows, int64_t seg_stride,
+                         int32_t K, int32_t N, int32_t C, int32_t PP, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * HBM-bound NHWC bf16 kernels around the convolutions.
@@ -195,12 +189,12 @@ int32_t c3d_bn_finalize(const float* partial, int32_t rows, int32_t C, double co
                         void* stream);
 /* out = [relu]((y-mean)*rstd*gamma+beta [+ residual]); y,out,residual bf16 (P pixels x C) */
 int32_t c3d_bn_apply(const void* y, const float* mean, const float* rstd, const float* gamma, const float* beta,
-                     const void* residual, int32_t relu, void* out, int64_t P, int32_t C, int64_t res_stride,
-                     int64_t out_stride, void* stream);
+                     const void* residual, int32_t relu, void* out, int64_t P, int32_t C, void* stream);
 /* rows of the `partial` scratch needed by c3d_bn_bwd */
 int32_t c3d_bn_bwd_blocks(int64_t P, int32_t C);
 /* BatchNorm(+ReLU,+residual) backward: dy (bf16) w.r.t. the conv output, dgamma/dbeta accumulated (+=),
  * optional dres = masked dout for the residual branch. partial: fp32 [blocks][2][C]; coef: fp32 [3][C].
+ * dout and dres may be channel slices of wider NHWC buffers: pixel strides dout_stride / dres_stride (0 => C).
  * frozen_stats != 0: mean/rstd are running statistics (eval mode / freeze_bn, cubercnn/solver/build.py:71-76).
  * out may be NULL for a ReLU layer WITHOUT residual when beta is given: the mask is then recomputed from y exactly as
  * c3d_bn_apply produced it (saves re-reading `out` in both passes).
@@ -210,8 +204,8 @@ int32_t c3d_bn_bwd_blocks(int64_t P, int32_t C);
 int32_t c3d_bn_bwd(const void* dout, const void* out, const void* y, const float* mean, const float* rstd,
                    const float* gamma, const float* beta, int32_t relu, int32_t frozen_stats, float* partial, float* coef, float* dgamma,
                    float* dbeta,
-                   void* dy, void* dres, int64_t P, int32_t C, int64_t dout_stride, int64_t out_stride,
-                   int64_t dres_stride, void* scratch, void* stream);
+                   void* dy, void* dres, int64_t P, int32_t C, int64_t dout_stride, int64_t dres_stride, void* scratch,
+                   void* stream);
 /* backward of the bias(+ReLU) epilogue of the bias convs (FPN / RPN head): dz (bf16) = dout * (out > 0 if relu),
  * dbias (fp32 [C]) += sum over pixels.  dtype_flags: bit 0 = dout is fp32 (else bf16), bit 1 = out is fp32 (else bf16).
  * partial: fp32 [c3d_bn_bwd_blocks(P,C)][C]; scratch: c3d_bn_scratch_bytes(C).
@@ -224,14 +218,12 @@ int32_t c3d_sumpool2(const void* x, void* y, int32_t N, int32_t H, int32_t W, in
 /* z (N,H,W,C) = dy (N,Ho,Wo,C) at even positions, zero elsewhere: input of a stride-2 conv's data gradient */
 int32_t c3d_zero_stuff2(const void* dy, void* z, int32_t N, int32_t Ho, int32_t Wo, int32_t H, int32_t W, int32_t C,
                         void* stream);
-int32_t c3d_maxpool2_fwd(const void* x, void* y, int32_t N, int32_t H, int32_t W, int32_t C, int64_t x_stride,
-                         int64_t y_stride, void* stream);
-int32_t c3d_maxpool2_bwd(const void* x, const void* dy, void* dx, int32_t N, int32_t H, int32_t W, int32_t C,
-                         int64_t x_stride, int64_t dy_stride, void* stream);
-/* same, accumulating: dx (pixel stride dx_stride, 0 => C) += routed dy — x feeds the pool AND a strided convolution
+int32_t c3d_maxpool2_fwd(const void* x, void* y, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
+/* dx (N,H,W,C) = dy (N,H/2,W/2,C) routed to the first maximal element of every 2x2 window; dy and dx have pixel strides
+ * dy_stride / dx_stride (0 => C).  accumulate != 0: dx += routed dy — x feeds the pool AND a strided convolution
  * (dla.py:209-214), the pool's share is added into the convolution's data gradient in place */
-int32_t c3d_maxpool2_bwd_acc(const void* x, const void* dy, void* dx, int32_t N, int32_t H, int32_t W, int32_t C,
-                             int64_t x_stride, int64_t dy_stride, int64_t dx_stride, void* stream);
+int32_t c3d_maxpool2_bwd(const void* x, const void* dy, void* dx, int32_t N, int32_t H, int32_t W, int32_t C,
+                         int64_t dy_stride, int64_t dx_stride, int32_t accumulate, void* stream);
 /* 3x3 / stride 2 / pad 1 max pool of the torchvision ResNet stem (cubercnn/modeling/backbone/resnet.py:17-27,45-50):
  * y (N,(H-1)/2+1,(W-1)/2+1,C); the backward routes dy to the first maximal element of every window (ATen tie order). */
 int32_t c3d_maxpool3s2_fwd(const void* x, void* y, int32_t N, int32_t H, int32_t W, int32_t C, void* stream);
@@ -245,20 +237,18 @@ int32_t c3d_preprocess_batch(const void* const* imgs_host, const int32_t* H_host
                              const float* std3_host, void* stream);
 /* flag |= 1 if any gradient element is NaN/Inf */
 int32_t c3d_grad_finite(const float* g, int64_t n, int32_t* flag, void* stream);
-/* torch.optim.SGD(momentum, weight_decay) over a flat arena; no-op if *skip_flag != 0 */
-int32_t c3d_sgd_momentum(float* p, const float* g, float* mom, int64_t n, float lr, float momentum,
+/* torch.optim.SGD(momentum, weight_decay) over a flat arena; no-op if *skip_flag != 0.  lr_dev (may be NULL): the
+ * learning rate read from device memory at run time instead of lr (schedule changes without re-recording a captured
+ * CUDA graph of the step) */
+int32_t c3d_sgd_momentum(float* p, const float* g, float* mom, int64_t n, float lr, const float* lr_dev, float momentum,
                          float weight_decay, float grad_scale, const int32_t* skip_flag, void* stream);
-/* same update with the learning rate read from device memory at run time (schedule changes without re-recording a
- * captured CUDA graph of the step) */
-int32_t c3d_sgd_momentum_dev(float* p, const float* g, float* mom, int64_t n, const float* lr_dev, float momentum,
-                             float weight_decay, float grad_scale, const int32_t* skip_flag, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Multi-level ROIAlign (aligned=True, sampling_ratio 0) on NHWC bf16 FPN maps.
  * Replaces detectron2 ROIPooler/ROIAlignV2 at cubercnn/modeling/roi_heads/roi_heads.py:267,362.
  * rois: fp32 [R][6] = (batch index, level index, x1, y1, x2, y2).  out: bf16 [R][ph][pw][C].
- * RoIs with a non-finite coordinate, a level outside [0, num_levels) or (when num_images > 0) an image index
- * outside [0, num_images) pool zeros / contribute no gradient instead of indexing out of bounds.
+ * RoIs with a non-finite coordinate, a level outside [0, num_levels) or an image index outside [0, num_images) pool
+ * zeros / contribute no gradient instead of indexing out of bounds.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
   const void* feat[5];   /* level l: bf16 (N,H[l],W[l],C) */
@@ -266,7 +256,7 @@ typedef struct {
   int32_t H[5], W[5];
   float scale[5];
   int32_t num_levels;
-  int32_t num_images;    /* N of the maps (0 = do not check the image index; c3d_roi_align_bwd requires it) */
+  int32_t num_images;    /* N of the maps (> 0) */
 } c3d_roi_levels;
 int32_t c3d_roi_align_fwd(const c3d_roi_levels* levels, const float* rois, int32_t R, int32_t C, int32_t pooled_h,
                           int32_t pooled_w, void* out, void* stream);

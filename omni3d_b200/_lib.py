@@ -24,7 +24,7 @@ class C3DError(RuntimeError):
 class ConvDesc(ctypes.Structure):
     _fields_ = [("N", i32), ("H", i32), ("W", i32), ("Cin", i32), ("Cout", i32), ("KH", i32), ("KW", i32),
                 ("stride", i32), ("pad", i32), ("relu", i32), ("out_fp32", i32), ("add_mode", i32),
-                ("x_pix_stride", i64), ("y_pix_stride", i64), ("add_pix_stride", i64),
+                ("y_pix_stride", i64),
                 ("y_img_stride", i64), ("y_h_stride", i64), ("y_w_stride", i64), ("y_offset", i64),
                 ("out_h", i32), ("out_w", i32), ("x_img_stride", i64), ("y_split_c", i32), ("pad_", i32),
                 ("y_split_off", i64)]
@@ -72,36 +72,30 @@ SIGNATURES = {
     # convolution
     "c3d_conv2d_tiles": (i32, [_conv, vp, vp, vp]),
     "c3d_conv2d_fwd": (i32, [_conv, vp, vp, vp, vp, vp, vp, vp]),
-    "c3d_conv2d_wgrad": (i32, [_conv, vp, vp, vp, vp]),
-    "c3d_conv2d_wgrad_ex": (i32, [_conv, vp, vp, vp, i32, vp]),
+    "c3d_conv2d_wgrad": (i32, [_conv, vp, vp, vp, i32, vp]),
     "c3d_pack_conv_weight": (i32, [ctypes.POINTER(PackDesc), vp]),
     "c3d_pack_conv_weights_batched": (i32, [vp, i32, i64, vp]),
     # fully-connected layers
     "c3d_pack_linear_weight": (i32, [vp, i32, i32, i32, i32, vp, vp, vp]),
-    "c3d_linear_fwd": (i32, [vp, vp, vp, vp, i64, i32, i32, i32, i32, vp]),
-    "c3d_linear_dgrad": (i32, [vp, vp, vp, i64, i32, i32, vp]),
-    "c3d_linear_wgrad": (i32, [vp, vp, vp, i64, i32, i32, i32, i32, i32, vp]),
-    "c3d_linear_fwd_blocks": (i32, [vp, vp, vp, vp, i32, i32, i64, i32, i32, i32, i32, vp]),
-    "c3d_linear_dgrad_blocks": (i32, [vp, vp, vp, i32, i32, i64, i32, i32, i32, vp]),
-    "c3d_linear_wgrad_blocks": (i32, [vp, vp, vp, i32, i32, i64, i32, i32, i32, i32, i32, vp]),
+    "c3d_linear_fwd": (i32, [vp, vp, vp, vp, i32, i64, i64, i32, i32, i32, i32, vp]),
+    "c3d_linear_dgrad": (i32, [vp, vp, vp, i32, i64, i64, i32, i32, i32, vp]),
+    "c3d_linear_wgrad": (i32, [vp, vp, vp, i32, i64, i64, i32, i32, i32, i32, vp]),
     # NHWC kernels around the convolutions
     "c3d_bn_scratch_bytes": (sz, [i32]),
     "c3d_bn_finalize": (i32, [vp, i32, i32, f64, f32, f32, vp, vp, vp, vp, vp, vp]),
-    "c3d_bn_apply": (i32, [vp, vp, vp, vp, vp, vp, i32, vp, i64, i32, i64, i64, vp]),
+    "c3d_bn_apply": (i32, [vp, vp, vp, vp, vp, vp, i32, vp, i64, i32, vp]),
     "c3d_bn_bwd_blocks": (i32, [i64, i32]),
-    "c3d_bn_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i64, i32, i64, i64, i64, vp, vp]),
+    "c3d_bn_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i64, i32, i64, i64, vp, vp]),
     "c3d_bias_act_bwd": (i32, [vp, vp, i32, i32, vp, vp, vp, i64, i32, vp, vp]),
     "c3d_sumpool2": (i32, [vp, vp, i32, i32, i32, i32, vp]),
     "c3d_zero_stuff2": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp]),
-    "c3d_maxpool2_fwd": (i32, [vp, vp, i32, i32, i32, i32, i64, i64, vp]),
-    "c3d_maxpool2_bwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i64, i64, vp]),
-    "c3d_maxpool2_bwd_acc": (i32, [vp, vp, vp, i32, i32, i32, i32, i64, i64, i64, vp]),
+    "c3d_maxpool2_fwd": (i32, [vp, vp, i32, i32, i32, i32, vp]),
+    "c3d_maxpool2_bwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i64, i64, i32, vp]),
     "c3d_maxpool3s2_fwd": (i32, [vp, vp, i32, i32, i32, i32, vp]),
     "c3d_maxpool3s2_bwd": (i32, [vp, vp, vp, i32, i32, i32, i32, i64, vp]),
     "c3d_preprocess_batch": (i32, [vp, vp, vp, i32, i32, vp, i32, i32, i32, vp, vp, vp]),
     "c3d_grad_finite": (i32, [vp, i64, vp, vp]),
-    "c3d_sgd_momentum": (i32, [vp, vp, vp, i64, f32, f32, f32, f32, vp, vp]),
-    "c3d_sgd_momentum_dev": (i32, [vp, vp, vp, i64, vp, f32, f32, f32, vp, vp]),
+    "c3d_sgd_momentum": (i32, [vp, vp, vp, i64, f32, vp, f32, f32, f32, vp, vp]),
     # ROIAlign
     "c3d_roi_align_fwd": (i32, [_roi, vp, i32, i32, i32, i32, vp, vp]),
     "c3d_roi_align_bwd": (i32, [_roi, vp, i32, i32, i32, i32, vp, vp]),

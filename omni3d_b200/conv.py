@@ -120,89 +120,71 @@ def conv2d_wgrad(x, dy, KH, KW, stride=1, pad=0, dw=None, oihw=False):
     if dw is None:
         dw = torch.zeros((Cout, Cin, KH, KW) if oihw else (Cout, KH, KW, Cin), device=x.device, dtype=torch.float32)
     d = ConvDesc(N=N, H=H, W=W, Cin=Cin, Cout=Cout, KH=KH, KW=KW, stride=stride, pad=pad)
-    _lib.check(L.c3d_conv2d_wgrad_ex(ctypes.byref(d), ptr(x), ptr(dy), ptr(dw), int(oihw), stream()))
+    _lib.check(L.c3d_conv2d_wgrad(ctypes.byref(d), ptr(x), ptr(dy), ptr(dw), int(oihw), stream()))
     return dw
 
 
 # ---- fully-connected layers on the same kernels (c3d_linear_*) -------------------------------------------------------
-def pack_linear_weight(w, chw=None, want_t=True):
-    """fp32 master (N, K) -> bf16 (N, K') [+ bf16 (K', N)].  chw = (C, PP): the master's input features are ordered
+def pack_linear_weight(w, chw=None):
+    """fp32 master (N, K) -> bf16 (N, K') and bf16 (K', N).  chw = (C, PP): the master's input features are ordered
     (c, p) (nn.Linear over an NCHW-flattened RoI) and are re-ordered to (p, c) (NHWC-flattened RoI)."""
     L = _lib.lib()
     N, Kdim = w.shape
     w = w.detach().contiguous()
     C, PP = chw if chw is not None else (Kdim, 1)
     f = torch.empty((N, Kdim), device=w.device, dtype=torch.bfloat16)
-    t = torch.empty((Kdim, N), device=w.device, dtype=torch.bfloat16) if want_t else None
-    _lib.check(L.c3d_pack_linear_weight(ptr(w), N, Kdim, C, PP, ptr(f), ptr(t), stream()), launches=2 if want_t else 1)
+    t = torch.empty((Kdim, N), device=w.device, dtype=torch.bfloat16)
+    _lib.check(L.c3d_pack_linear_weight(ptr(w), N, Kdim, C, PP, ptr(f), ptr(t), stream()), launches=2)
     return f, t
 
 
-def linear_fwd(x, w, bias=None, relu=False, out_fp32=False):
-    """x (rows, K) bf16, w (N, K) bf16, bias (N,) fp32 -> [relu](x w^T + bias) (rows, N) bf16 | fp32."""
-    L = _lib.lib()
-    rows, Kdim = x.shape
-    N = w.shape[0]
-    assert x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.is_contiguous() and w.is_contiguous()
-    assert w.shape[1] == Kdim and (bias is None or (bias.dtype == torch.float32 and bias.is_contiguous()))
-    y = torch.empty((rows, N), device=x.device, dtype=torch.float32 if out_fp32 else torch.bfloat16)
-    _lib.check(L.c3d_linear_fwd(ptr(x), ptr(w), ptr(bias), ptr(y), rows, Kdim, N, int(relu), int(out_fp32), stream()))
-    return y
+def _row_blocks(m, blocks):
+    """(nseg, seg_rows, seg_stride) of the c3d_linear_* row blocks inside the (rows, ..) matrix m; blocks None: all rows"""
+    rows = m.shape[0]
+    nseg, seg_rows, seg_stride = blocks if blocks is not None else (1, rows, rows)
+    assert (nseg - 1) * seg_stride + seg_rows <= rows, (blocks, tuple(m.shape))
+    return nseg, seg_rows, seg_stride
 
 
-def linear_dgrad(dy, wt):
-    """dy (rows, N) bf16, wt (K, N) bf16 (the transposed weight) -> dx (rows, K) bf16."""
-    L = _lib.lib()
-    rows, N = dy.shape
-    Kdim = wt.shape[0]
-    assert dy.dtype == torch.bfloat16 and wt.dtype == torch.bfloat16 and dy.is_contiguous() and wt.is_contiguous()
-    dx = torch.empty((rows, Kdim), device=dy.device, dtype=torch.bfloat16)
-    _lib.check(L.c3d_linear_dgrad(ptr(dy), ptr(wt), ptr(dx), rows, N, Kdim, stream()))
-    return dx
-
-
-def linear_wgrad(x, dy, dw=None, chw=None, master_chw=True):
-    """dw (N, K) fp32 (+)= dy^T x.  chw = (C, PP) + master_chw: address dw in the master's (c, p) feature order."""
-    L = _lib.lib()
-    rows, Kdim = x.shape
-    N = dy.shape[1]
-    assert x.dtype == torch.bfloat16 and dy.dtype == torch.bfloat16 and x.is_contiguous() and dy.is_contiguous()
-    if dw is None:
-        dw = torch.zeros((N, Kdim), device=x.device, dtype=torch.float32)
-    C, PP = chw if chw is not None else (Kdim, 1)
-    _lib.check(L.c3d_linear_wgrad(ptr(x), ptr(dy), ptr(dw), rows, Kdim, N, C, PP, int(bool(master_chw and chw is not None)),
-                                  stream()))
-    return dw
-
-
-def linear_fwd_blocks(x, nseg, seg_rows, seg_stride, w, bias=None, relu=False, out_fp32=False):
-    """rows [b*seg_stride, b*seg_stride + seg_rows) of x (.., K), b < nseg, read in place -> dense (nseg*seg_rows, N)."""
+def linear_fwd(x, w, bias=None, relu=False, out_fp32=False, blocks=None):
+    """x (rows, K) bf16, w (N, K) bf16, bias (N,) fp32 -> [relu](x w^T + bias) (rows, N) bf16 | fp32.
+    blocks = (nseg, seg_rows, seg_stride): only rows [b*seg_stride, b*seg_stride + seg_rows) of x, b < nseg, read in
+    place -> (nseg*seg_rows, N)."""
     L = _lib.lib()
     Kdim, N = x.shape[1], w.shape[0]
-    assert x.dtype == torch.bfloat16 and x.is_contiguous() and w.is_contiguous() and (nseg - 1) * seg_stride + seg_rows <= x.shape[0]
+    nseg, seg_rows, seg_stride = _row_blocks(x, blocks)
+    assert x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.is_contiguous() and w.is_contiguous()
+    assert w.shape[1] == Kdim and (bias is None or (bias.dtype == torch.float32 and bias.is_contiguous()))
     y = torch.empty((nseg * seg_rows, N), device=x.device, dtype=torch.float32 if out_fp32 else torch.bfloat16)
-    _lib.check(L.c3d_linear_fwd_blocks(ptr(x), ptr(w), ptr(bias), ptr(y), nseg, seg_rows, seg_stride, Kdim, N, int(relu),
-                                       int(out_fp32), stream()))
+    _lib.check(L.c3d_linear_fwd(ptr(x), ptr(w), ptr(bias), ptr(y), nseg, seg_rows, seg_stride, Kdim, N, int(relu),
+                                int(out_fp32), stream()))
     return y
 
 
-def linear_dgrad_blocks(dy, wt, dx, nseg, seg_rows, seg_stride, accumulate=True):
-    """dx rows [b*seg_stride, +seg_rows) (+)= dy (nseg*seg_rows, N) . W, in place inside the larger dx (.., K)."""
+def linear_dgrad(dy, wt, blocks=None, dx=None, accumulate=False):
+    """dy (rows, N) bf16, wt (K, N) bf16 (the transposed weight) -> dx (rows, K) bf16 = dy . W.  dx: write into this
+    buffer instead, at rows [b*seg_stride, +seg_rows) of blocks = (nseg, seg_rows, seg_stride); accumulate: dx +=."""
     L = _lib.lib()
     N, Kdim = dy.shape[1], wt.shape[0]
-    assert dy.dtype == torch.bfloat16 and dy.is_contiguous() and dx.dtype == torch.bfloat16 and dx.is_contiguous()
-    assert dx.shape[1] == Kdim and (nseg - 1) * seg_stride + seg_rows <= dx.shape[0] and dy.shape[0] == nseg * seg_rows
-    _lib.check(L.c3d_linear_dgrad_blocks(ptr(dy), ptr(wt), ptr(dx), nseg, seg_rows, seg_stride, N, Kdim, int(accumulate), stream()))
+    assert dy.dtype == torch.bfloat16 and wt.dtype == torch.bfloat16 and dy.is_contiguous() and wt.is_contiguous()
+    if dx is None:
+        dx = torch.empty((dy.shape[0], Kdim), device=dy.device, dtype=torch.bfloat16)
+    nseg, seg_rows, seg_stride = _row_blocks(dx, blocks)
+    assert dx.dtype == torch.bfloat16 and dx.is_contiguous() and dx.shape[1] == Kdim and dy.shape[0] == nseg * seg_rows
+    _lib.check(L.c3d_linear_dgrad(ptr(dy), ptr(wt), ptr(dx), nseg, seg_rows, seg_stride, N, Kdim, int(accumulate),
+                                  stream()))
     return dx
 
 
-def linear_wgrad_blocks(x, dy, nseg, seg_rows, seg_stride, dw=None, chw=None, master_chw=True):
+def linear_wgrad(x, dy, dw=None, chw=None, blocks=None):
+    """dw (N, K) fp32 (+)= dy^T x over the rows of x that blocks selects (as in linear_fwd).  chw = (C, PP): x's features
+    are the (p, c) re-ordering of the master's (c, p) ones (pack_linear_weight), and dw is addressed in the master's order."""
     L = _lib.lib()
     Kdim, N = x.shape[1], dy.shape[1]
+    nseg, seg_rows, seg_stride = _row_blocks(x, blocks)
     assert x.dtype == torch.bfloat16 and dy.dtype == torch.bfloat16 and x.is_contiguous() and dy.is_contiguous()
     if dw is None:
         dw = torch.zeros((N, Kdim), device=x.device, dtype=torch.float32)
     C, PP = chw if chw is not None else (Kdim, 1)
-    _lib.check(L.c3d_linear_wgrad_blocks(ptr(x), ptr(dy), ptr(dw), nseg, seg_rows, seg_stride, Kdim, N, C, PP,
-                                         int(bool(master_chw and chw is not None)), stream()))
+    _lib.check(L.c3d_linear_wgrad(ptr(x), ptr(dy), ptr(dw), nseg, seg_rows, seg_stride, Kdim, N, C, PP, stream()))
     return dw

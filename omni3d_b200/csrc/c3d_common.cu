@@ -14,4 +14,4 @@ int32_t set_error(int32_t code, const char* fmt, ...) {
 }  // namespace c3d
 
 extern "C" const char* c3d_last_error(void) { return c3d::last_error_buf(); }
-extern "C" int32_t c3d_abi_version(void) { return 3; }
+extern "C" int32_t c3d_abi_version(void) { return 4; }

@@ -391,7 +391,6 @@ static bool halo_fwd_eligible(const c3d_conv_desc* d) {
   if (d->out_h > 0 || d->out_w > 0 || d->add_mode != 0) return false;
   if (!(d->Cin == 8 || d->Cin == 16 || d->Cin == 32)) return false;
   if (!(d->Cout == 16 || d->Cout == 32)) return false;
-  if (d->x_pix_stride != 0 && d->x_pix_stride != d->Cin) return false;
   if ((d->W < 128 && d->Cin != 8) || d->KH > 7) return false;   // NHWC8 input exists only for this kernel
   return true;
 }
@@ -399,7 +398,7 @@ static bool halo_wgrad_eligible(const c3d_conv_desc* d) {
   if (d->stride != 1 || d->KH != d->KW || !(d->KH & 1) || 2 * d->pad != d->KH - 1) return false;
   if (!(d->Cin == 8 || d->Cin == 16 || d->Cin == 32)) return false;
   if (!(d->Cout == 16 || d->Cout == 32)) return false;
-  if ((d->x_pix_stride != 0 && d->x_pix_stride != d->Cin) || (d->y_pix_stride != 0 && d->y_pix_stride != d->Cout)) return false;
+  if (d->y_pix_stride != 0 && d->y_pix_stride != d->Cout) return false;
   if (d->W < 128 && d->Cin != 8) return false;
   return (d->KH == 7 && d->Cin == 8) || (d->KH == 3 && d->Cin >= 16);     // the compiled instances
 }

@@ -37,9 +37,8 @@ struct ConvKParams {
   const float* bias;         // [Cout] or null
   int relu;
   int out_fp32;
-  int add_mode;              // 0 none, 1 same-size, 2 nearest-up2 (addend (N,Ho/2,Wo/2,add_pix_stride)), 3 in place
+  int add_mode;              // 0 none, 1 same-size, 2 nearest-up2 (addend (N,Ho/2,Wo/2,Cout)), 3 in place
   const bf16* addend;
-  long long add_pix_stride;
   void* out;
   long long out_pix_stride;  // elements
   long long out_img_stride, out_h_stride, out_w_stride, out_off;   // output pixel index = img*is + ho*hs + wo*ws + off
@@ -111,7 +110,7 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvKParams& P, const f
       float v0 = acc[4 * j + 2 * h] + bv.x, v1 = acc[4 * j + 2 * h + 1] + bv.y;
       if (P.add_mode) {
         const bf16* ap = P.add_mode == 3 ? reinterpret_cast<const bf16*>(P.out) + pix[h] * P.out_pix_stride + coff
-                                         : P.addend + apix[h] * P.add_pix_stride + c;
+                                         : P.addend + apix[h] * P.Cout + c;
         const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(ap));
         v0 += a.x; v1 += a.y;
       }
@@ -563,7 +562,6 @@ extern "C" int32_t c3d_conv2d_fwd(const c3d_conv_desc* d, const void* x, const v
   P.kc_blocks = Cin / BK; P.Cin = Cin;
   P.bias = bias; P.relu = d->relu; P.out_fp32 = d->out_fp32; P.add_mode = d->add_mode;
   P.addend = static_cast<const bf16*>(addend);
-  P.add_pix_stride = d->add_pix_stride ? d->add_pix_stride : Cout;
   P.out = y; P.out_pix_stride = d->y_pix_stride ? d->y_pix_stride : Cout;
   if (d->y_img_stride) {
     P.out_img_stride = d->y_img_stride; P.out_h_stride = d->y_h_stride; P.out_w_stride = d->y_w_stride; P.out_off = d->y_offset;
@@ -572,13 +570,12 @@ extern "C" int32_t c3d_conv2d_fwd(const c3d_conv_desc* d, const void* x, const v
   }
   P.split_c = d->y_split_c; P.split_off = d->y_split_off;
   P.stats = stats;
-  const long long xps = d->x_pix_stride ? d->x_pix_stride : Cin;
 
   CUtensorMap mx, mw;
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N};
-    cuuint64_t strides[3] = {(cuuint64_t)xps * 2, (cuuint64_t)xps * 2 * d->W,
-                             (cuuint64_t)xps * 2 * (d->x_img_stride ? d->x_img_stride : (long long)d->W * d->H)};
+    cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cin * 2 * d->W,
+                             (cuuint64_t)Cin * 2 * (d->x_img_stride ? d->x_img_stride : (long long)d->W * d->H)};
     cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)(P.TW * d->stride), (cuuint32_t)(P.TH * d->stride), 1};
     cuuint32_t estr[4] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1};
     CUresult r = enc(&mx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
@@ -620,20 +617,9 @@ extern "C" int32_t c3d_conv2d_fwd(const c3d_conv_desc* d, const void* x, const v
   return set_error(C3D_EINVAL, "conv2d: no kernel for BN=%d BK=%d", BN, BK);
 }
 
-extern "C" int32_t c3d_conv2d_wgrad_ex(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int32_t oihw,
-                                       void* stream);
-extern "C" int32_t c3d_conv2d_wgrad(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, void* stream) {
-  return c3d_conv2d_wgrad_ex(d, x, dy, dw, 0, stream);
-}
 // lin_c > 0: fully-connected layer — d describes the layer as a 1x1 conv over (1,1,rows) "pixels" with d->Cin input
 // features that are laid out as (lin_pp taps) x (lin_c channels); the epilogue then addresses dw as [Cout][lin_c][lin_pp]
 // when oihw (the nn.Linear master weight over a (C,P,P)-flattened input) or [Cout][lin_pp][lin_c] otherwise.
-static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int32_t oihw, void* stream,
-                          int lin_c, int lin_pp);
-extern "C" int32_t c3d_conv2d_wgrad_ex(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int32_t oihw,
-                                       void* stream) {
-  return wgrad_impl(d, x, dy, dw, oihw, stream, 0, 0);
-}
 static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int32_t oihw, void* stream,
                           int lin_c, int lin_pp) {
   if (!d || !x || !dy || !dw) return set_error(C3D_EINVAL, "wgrad: null pointer");
@@ -680,7 +666,6 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   P.part = nullptr;
   P.welems = welems;
   P.oihw = oihw;
-  const long long xps = d->x_pix_stride ? d->x_pix_stride : Cin;
   const long long yps = d->y_pix_stride ? d->y_pix_stride : Cout;
   CUtensorMap mdy, mx;
   // 5-D maps (channel-chunk axis OUTSIDE the pixel axes): one box = [chunks][RH][RW][64 ch], the MN-major operand layout
@@ -697,7 +682,7 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
     cuuint32_t dy_box[5] = {(cuuint32_t)P.ca, (cuuint32_t)P.RW, (cuuint32_t)P.RH, (cuuint32_t)P.a_chunks_max, 1};
     cuuint32_t one5[5] = {1, 1, 1, 1, 1};
     cuuint64_t x_dims[5] = {(cuuint64_t)P.cw, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)nchunks_x, (cuuint64_t)d->N};
-    cuuint64_t x_str[4] = {(cuuint64_t)xps * 2, (cuuint64_t)xps * 2 * d->W, (cuuint64_t)P.cw * 2, (cuuint64_t)xps * 2 * ximg};
+    cuuint64_t x_str[4] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cin * 2 * d->W, (cuuint64_t)P.cw * 2, (cuuint64_t)Cin * 2 * ximg};
     cuuint32_t x_box[5] = {(cuuint32_t)P.cw, (cuuint32_t)(P.RW * d->stride), (cuuint32_t)(P.RH * d->stride), (cuuint32_t)mc, 1};
     cuuint32_t x_es[5] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1, 1};
     CUresult r1 = enc(&mdy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(dy), dy_dims, dy_str, dy_box, one5,
@@ -725,8 +710,8 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   }
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N};
-    cuuint64_t strides[3] = {(cuuint64_t)xps * 2, (cuuint64_t)xps * 2 * d->W,
-                             (cuuint64_t)xps * 2 * (d->x_img_stride ? d->x_img_stride : (long long)d->W * d->H)};
+    cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cin * 2 * d->W,
+                             (cuuint64_t)Cin * 2 * (d->x_img_stride ? d->x_img_stride : (long long)d->W * d->H)};
     cuuint32_t box[4] = {(cuuint32_t)P.cw, (cuuint32_t)(P.RW * d->stride), (cuuint32_t)(P.RH * d->stride), 1};
     cuuint32_t estr[4] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1};
     CUresult r = enc(&mx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
@@ -750,6 +735,11 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
     conv_wgrad_tc_kernel<<<grid, kGemmThreads, WgradSmem::kTotal, st>>>(mdy, mx, Q);
     return check_launch("conv_wgrad_tc_kernel");
   });
+}
+
+extern "C" int32_t c3d_conv2d_wgrad(const c3d_conv_desc* d, const void* x, const void* dy, float* dw, int32_t oihw,
+                                    void* stream) {
+  return wgrad_impl(d, x, dy, dw, oihw, stream, 0, 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -789,87 +779,58 @@ __global__ void transpose_bf16_kernel(const bf16* __restrict__ in, int R, int Cc
       if (c < Cc && r0 + j < R) out[(size_t)c * R + r0 + j] = t[j][i];
   }
 }
-static void linear_desc(c3d_conv_desc* d, int64_t rows, int K, int N, int relu, int out_fp32) {
+// the layer over nseg blocks of seg_rows rows as a 1x1 convolution of nseg (1, seg_rows) "images" with K input and N
+// output channels; block b starts at row b * seg_stride of the strided operand, which the caller places.  d->N == 0:
+// nothing to compute.
+static int32_t linear_desc(c3d_conv_desc* d, int32_t nseg, int64_t seg_rows, int64_t seg_stride, int K, int N) {
   memset(d, 0, sizeof(*d));
-  d->N = 1; d->H = 1; d->W = (int32_t)rows; d->Cin = K; d->Cout = N; d->KH = 1; d->KW = 1; d->stride = 1; d->pad = 0;
-  d->relu = relu; d->out_fp32 = out_fp32;
+  if (nseg <= 0 || seg_rows <= 0) return C3D_OK;
+  if (seg_rows > 0x7fffffffLL) return set_error(C3D_EINVAL, "linear: seg_rows %lld exceeds INT32_MAX", (long long)seg_rows);
+  if (seg_stride < seg_rows) return set_error(C3D_EINVAL, "linear: seg_stride < seg_rows");
+  d->N = nseg; d->H = 1; d->W = (int32_t)seg_rows; d->Cin = K; d->Cout = N; d->KH = 1; d->KW = 1; d->stride = 1; d->pad = 0;
+  return C3D_OK;
 }
 }  // namespace c3d
 
 extern "C" int32_t c3d_pack_linear_weight(const float* w, int32_t N, int32_t K, int32_t C, int32_t PP, void* w_bf16,
                                           void* wt_bf16, void* stream) {
-  if (!w || !w_bf16 || N <= 0 || K <= 0) return set_error(C3D_EINVAL, "pack_linear_weight: bad args");
+  if (!w || !w_bf16 || !wt_bf16 || N <= 0 || K <= 0) return set_error(C3D_EINVAL, "pack_linear_weight: bad args");
   if (C <= 0 || PP <= 0) { C = K; PP = 1; }
   if ((long long)C * PP != K || PP > 256) return set_error(C3D_EINVAL, "pack_linear_weight: C*PP != K");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   dim3 g((C + 63) / 64, N);
   pack_linear_rows_kernel<<<g, 256, 64 * PP * sizeof(float), st>>>(w, N, C, PP, (bf16*)w_bf16);
-  if (wt_bf16) {
-    dim3 gt((K + 63) / 64, (N + 63) / 64);
-    transpose_bf16_kernel<<<gt, dim3(32, 8), 0, st>>>((const bf16*)w_bf16, N, K, (bf16*)wt_bf16);
-  }
+  dim3 gt((K + 63) / 64, (N + 63) / 64);
+  transpose_bf16_kernel<<<gt, dim3(32, 8), 0, st>>>((const bf16*)w_bf16, N, K, (bf16*)wt_bf16);
   return check_launch("pack_linear_weight");
 }
 
-extern "C" int32_t c3d_linear_fwd(const void* x, const void* w, const float* bias, void* y, int64_t rows, int32_t K,
-                                  int32_t N, int32_t relu, int32_t out_fp32, void* stream) {
-  if (rows <= 0) return C3D_OK;
-  if (rows > 0x7fffffffLL) return set_error(C3D_EINVAL, "linear: too many rows");
+extern "C" int32_t c3d_linear_fwd(const void* x, const void* w, const float* bias, void* y, int32_t nseg, int64_t seg_rows,
+                                  int64_t seg_stride, int32_t K, int32_t N, int32_t relu, int32_t out_fp32, void* stream) {
   c3d_conv_desc d;
-  linear_desc(&d, rows, K, N, relu, out_fp32);
+  const int32_t rc = linear_desc(&d, nseg, seg_rows, seg_stride, K, N);
+  if (rc != C3D_OK || d.N == 0) return rc;
+  d.x_img_stride = seg_stride;
+  d.relu = relu; d.out_fp32 = out_fp32;
   return c3d_conv2d_fwd(&d, x, w, bias, nullptr, y, nullptr, stream);
 }
 
-extern "C" int32_t c3d_linear_dgrad(const void* dy, const void* wt, void* dx, int64_t rows, int32_t N, int32_t K,
-                                    void* stream) {
-  if (rows <= 0) return C3D_OK;
-  if (rows > 0x7fffffffLL) return set_error(C3D_EINVAL, "linear: too many rows");
+extern "C" int32_t c3d_linear_dgrad(const void* dy, const void* wt, void* dx, int32_t nseg, int64_t seg_rows,
+                                    int64_t seg_stride, int32_t N, int32_t K, int32_t accumulate, void* stream) {
   c3d_conv_desc d;
-  linear_desc(&d, rows, N, K, 0, 0);           // dx (rows, K) = dy (rows, N) . W  ==  1x1 conv with weight W^T (K, N)
-  return c3d_conv2d_fwd(&d, dy, wt, nullptr, nullptr, dx, nullptr, stream);
-}
-
-extern "C" int32_t c3d_linear_fwd_blocks(const void* x, const void* w, const float* bias, void* y, int32_t nseg,
-                                         int32_t seg_rows, int64_t seg_stride, int32_t K, int32_t N, int32_t relu,
-                                         int32_t out_fp32, void* stream) {
-  if (nseg <= 0 || seg_rows <= 0) return C3D_OK;
-  if (seg_stride < seg_rows) return set_error(C3D_EINVAL, "linear blocks: seg_stride < seg_rows");
-  c3d_conv_desc d;
-  linear_desc(&d, seg_rows, K, N, relu, out_fp32);
-  d.N = nseg; d.x_img_stride = seg_stride;
-  return c3d_conv2d_fwd(&d, x, w, bias, nullptr, y, nullptr, stream);
-}
-
-extern "C" int32_t c3d_linear_dgrad_blocks(const void* dy, const void* wt, void* dx, int32_t nseg, int32_t seg_rows,
-                                           int64_t seg_stride, int32_t N, int32_t K, int32_t accumulate, void* stream) {
-  if (nseg <= 0 || seg_rows <= 0) return C3D_OK;
-  if (seg_stride < seg_rows) return set_error(C3D_EINVAL, "linear blocks: seg_stride < seg_rows");
-  c3d_conv_desc d;
-  linear_desc(&d, seg_rows, N, K, 0, 0);
-  d.N = nseg;
-  d.y_img_stride = seg_stride; d.y_h_stride = seg_rows; d.y_w_stride = 1; d.y_offset = 0;   // rows of block b start at b*seg_stride
+  const int32_t rc = linear_desc(&d, nseg, seg_rows, seg_stride, N, K);   // dx = dy . W: 1x1 conv with weight W^T (K, N)
+  if (rc != C3D_OK || d.N == 0) return rc;
+  d.y_img_stride = seg_stride; d.y_h_stride = seg_rows; d.y_w_stride = 1; d.y_offset = 0;
   d.add_mode = accumulate ? 3 : 0;
   return c3d_conv2d_fwd(&d, dy, wt, nullptr, nullptr, dx, nullptr, stream);
 }
 
-extern "C" int32_t c3d_linear_wgrad_blocks(const void* x, const void* dy, float* dw, int32_t nseg, int32_t seg_rows,
-                                           int64_t seg_stride, int32_t K, int32_t N, int32_t C, int32_t PP,
-                                           int32_t master_chw, void* stream) {
-  if (nseg <= 0 || seg_rows <= 0) return C3D_OK;
-  if (seg_stride < seg_rows) return set_error(C3D_EINVAL, "linear blocks: seg_stride < seg_rows");
-  if (C <= 0 || PP <= 0) { C = K; PP = 1; }
+extern "C" int32_t c3d_linear_wgrad(const void* x, const void* dy, float* dw, int32_t nseg, int64_t seg_rows,
+                                    int64_t seg_stride, int32_t K, int32_t N, int32_t C, int32_t PP, void* stream) {
   c3d_conv_desc d;
-  linear_desc(&d, seg_rows, K, N, 0, 0);
-  d.N = nseg; d.x_img_stride = seg_stride;
-  return wgrad_impl(&d, x, dy, dw, master_chw ? 1 : 0, stream, C, PP);
-}
-
-extern "C" int32_t c3d_linear_wgrad(const void* x, const void* dy, float* dw, int64_t rows, int32_t K, int32_t N,
-                                    int32_t C, int32_t PP, int32_t master_chw, void* stream) {
-  if (rows <= 0) return C3D_OK;
-  if (rows > 0x7fffffffLL) return set_error(C3D_EINVAL, "linear: too many rows");
+  const int32_t rc = linear_desc(&d, nseg, seg_rows, seg_stride, K, N);
+  if (rc != C3D_OK || d.N == 0) return rc;
+  d.x_img_stride = seg_stride;
   if (C <= 0 || PP <= 0) { C = K; PP = 1; }
-  c3d_conv_desc d;
-  linear_desc(&d, rows, K, N, 0, 0);
-  return wgrad_impl(&d, x, dy, dw, master_chw ? 1 : 0, stream, C, PP);
+  return wgrad_impl(&d, x, dy, dw, PP > 1, stream, C, PP);
 }

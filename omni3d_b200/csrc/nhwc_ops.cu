@@ -84,7 +84,7 @@ __device__ __forceinline__ void slab_sums(const double* slab, int slabs, size_t 
 __global__ void __launch_bounds__(256)
 bn_apply_kernel(const bf16* __restrict__ y, const float* __restrict__ mean, const float* __restrict__ rstd,
                 const float* __restrict__ gamma, const float* __restrict__ beta, const bf16* __restrict__ residual, int relu,
-                bf16* __restrict__ out, long long P, int C, long long res_stride, long long out_stride) {
+                bf16* __restrict__ out, long long P, int C) {
   const int cv = C >> 3;
   const int tx = threadIdx.x % cv, ty = threadIdx.x / cv;
   const int rows_per_block = blockDim.x / cv;
@@ -98,7 +98,7 @@ bn_apply_kernel(const bf16* __restrict__ y, const float* __restrict__ mean, cons
     V8 a = ld8(y + p * C + c);
     V8 o;
     if (residual) {
-      V8 r = ld8(residual + p * res_stride + c);
+      V8 r = ld8(residual + p * C + c);
 #pragma unroll
       for (int k = 0; k < 8; ++k) o.v[k] = __fmaf_rn(a.v[k] - m[k], sc[k], bt[k]) + r.v[k];
     } else {
@@ -109,7 +109,7 @@ bn_apply_kernel(const bf16* __restrict__ y, const float* __restrict__ mean, cons
 #pragma unroll
       for (int k = 0; k < 8; ++k) o.v[k] = fmaxf(o.v[k], 0.f);
     }
-    st8(out + p * out_stride + c, o);
+    st8(out + p * C + c, o);
   }
 }
 
@@ -144,7 +144,7 @@ template <int THREADS>
 __global__ void __launch_bounds__(THREADS, 4)
 bn_bwd_reduce_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ out, const bf16* __restrict__ y,
                      const float* __restrict__ mean, const float* __restrict__ rstd, int relu, float* __restrict__ partial,
-                     long long P, int C, long long dout_stride, long long out_stride, const float* __restrict__ gamma,
+                     long long P, int C, long long dout_stride, const float* __restrict__ gamma,
                      const float* __restrict__ beta) {
   // `out == nullptr` with relu: the layer has no residual, so its ReLU mask is a function of y alone
   __shared__ float cm[3 * kBnMaxC];
@@ -159,13 +159,14 @@ bn_bwd_reduce_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ out
   float s[8], t[8];
 #pragma unroll
   for (int k = 0; k < 8; ++k) { s[k] = 0.f; t[k] = 0.f; }
+  const bf16* yc = y + c;          // hoisted: the loop then fits the 64-register bound of 4 CTAs per SM without spilling
   if (ty < rows_per_block) {
     for (long long p = (long long)blockIdx.x * rows_per_block + ty; p < P; p += (long long)gridDim.x * rows_per_block) {
       V8 d = ld8(dout + p * dout_stride + c);
-      const V8 yy = ld8(y + p * C + c);
+      const V8 yy = ld8(yc + p * C);
       if (remask) bn_remask(d, yy, cm, c);
       else if (relu) {
-        const V8 o = ld8(out + p * out_stride + c);
+        const V8 o = ld8(out + p * C + c);
 #pragma unroll
         for (int k = 0; k < 8; ++k) if (!(o.v[k] > 0.f)) d.v[k] = 0.f;
       }
@@ -192,7 +193,7 @@ __global__ void __launch_bounds__(256, 4)
 bn_bwd_apply_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ out, const bf16* __restrict__ y,
                     const float* __restrict__ mean, const float* __restrict__ rstd, const float* __restrict__ coef, int relu,
                     bf16* __restrict__ dy, bf16* __restrict__ dres, long long P, int C, long long dout_stride,
-                    long long out_stride, long long dres_stride, const float* __restrict__ gamma,
+                    long long dres_stride, const float* __restrict__ gamma,
                     const float* __restrict__ beta, int dres_acc) {
   __shared__ float cm[3 * kBnMaxC];
   const bool remask = relu && out == nullptr;
@@ -212,7 +213,7 @@ bn_bwd_apply_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ out,
     const V8 yy = ld8(y + p * C + c);
     if (remask) bn_remask(d, yy, cm, c);
     else if (relu) {
-      const V8 o = ld8(out + p * out_stride + c);
+      const V8 o = ld8(out + p * C + c);
 #pragma unroll
       for (int k = 0; k < 8; ++k) if (!(o.v[k] > 0.f)) d.v[k] = 0.f;
     }
@@ -417,8 +418,7 @@ __global__ void zero_stuff2_kernel(const bf16* __restrict__ dy, bf16* __restrict
 }
 
 // ---- 2x2 stride-2 max pool (NHWC) -------------------------------------------------------------
-__global__ void maxpool2_fwd_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, int N, int H, int W, int C,
-                                    long long x_stride, long long y_stride) {
+__global__ void maxpool2_fwd_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, int N, int H, int W, int C) {
   const int Ho = H >> 1, Wo = W >> 1, cv = C >> 3;
   const long long total = (long long)N * Ho * Wo * cv;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
@@ -429,19 +429,18 @@ __global__ void maxpool2_fwd_kernel(const bf16* __restrict__ x, bf16* __restrict
     const int ho = (int)(p % Ho);
     const int n = (int)(p / Ho);
     const long long base = ((long long)n * H + 2 * ho) * W + 2 * wo;
-    V8 a = ld8(x + base * x_stride + c), b = ld8(x + (base + 1) * x_stride + c);
-    V8 d = ld8(x + (base + W) * x_stride + c), e = ld8(x + (base + W + 1) * x_stride + c);
+    V8 a = ld8(x + base * C + c), b = ld8(x + (base + 1) * C + c);
+    V8 d = ld8(x + (base + W) * C + c), e = ld8(x + (base + W + 1) * C + c);
     V8 o;
 #pragma unroll
     for (int k = 0; k < 8; ++k) o.v[k] = fmaxf(fmaxf(a.v[k], b.v[k]), fmaxf(d.v[k], e.v[k]));
-    st8(y + (((long long)n * Ho + ho) * Wo + wo) * y_stride + c, o);
+    st8(y + (((long long)n * Ho + ho) * Wo + wo) * C + c, o);
   }
 }
 // dx (N,H,W,C) = dy routed to the first maximal element of each window (row-major window order)
 template <bool ACC>
 __global__ void maxpool2_bwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ dy, bf16* __restrict__ dx,
-                                    int N, int H, int W, int C, long long x_stride, long long dy_stride,
-                                    long long dx_stride) {
+                                    int N, int H, int W, int C, long long dy_stride, long long dx_stride) {
   const int Ho = H >> 1, Wo = W >> 1, cv = C >> 3;
   const long long total = (long long)N * Ho * Wo * cv;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
@@ -455,7 +454,7 @@ __global__ void maxpool2_bwd_kernel(const bf16* __restrict__ x, const bf16* __re
     const long long off[4] = {base, base + 1, base + W, base + W + 1};
     V8 v[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) v[j] = ld8(x + off[j] * x_stride + c);
+    for (int j = 0; j < 4; ++j) v[j] = ld8(x + off[j] * C + c);
     V8 g = ld8(dy + (((long long)n * Ho + ho) * Wo + wo) * dy_stride + c);
     V8 o[4];
 #pragma unroll
@@ -680,13 +679,12 @@ extern "C" int32_t c3d_bn_finalize(const float* partial, int32_t rows, int32_t C
 }
 extern "C" int32_t c3d_bn_apply(const void* y, const float* mean, const float* rstd, const float* gamma,
                                 const float* beta, const void* residual, int32_t relu, void* out, int64_t P,
-                                int32_t C, int64_t res_stride, int64_t out_stride, void* stream) {
+                                int32_t C, void* stream) {
   C3D_REQ(y && mean && rstd && gamma && beta && out && C % 8 == 0, "bn_apply: bad args");
   if (P == 0) return C3D_OK;
   C3D_REQ(C <= 2048, "bn_apply: C too large");
   bn_apply_kernel<<<grid_for(P * (C / 8), 256), 256, 0, (cudaStream_t)stream>>>(
-      (const bf16*)y, mean, rstd, gamma, beta, (const bf16*)residual, relu, (bf16*)out, P, C,
-      res_stride ? res_stride : C, out_stride ? out_stride : C);
+      (const bf16*)y, mean, rstd, gamma, beta, (const bf16*)residual, relu, (bf16*)out, P, C);
   return check_launch("bn_apply");
 }
 extern "C" int32_t c3d_bn_bwd_blocks(int64_t P, int32_t C) {
@@ -701,8 +699,7 @@ extern "C" int32_t c3d_bn_bwd(const void* dout, const void* out, const void* y, 
                               const float* gamma, const float* beta, int32_t relu, int32_t frozen_stats,
                               float* partial /*[blocks][2][C]*/, float* coef /*[3][C]*/,
                               float* dgamma, float* dbeta, void* dy, void* dres, int64_t P, int32_t C,
-                              int64_t dout_stride, int64_t out_stride, int64_t dres_stride, void* scratch,
-                              void* stream) {
+                              int64_t dout_stride, int64_t dres_stride, void* scratch, void* stream) {
   const int dres_acc = (relu >> 1) & 1;          // flags: bit 0 = ReLU, bit 1 = dres += (instead of =)
   relu &= 1;
   C3D_REQ(dout && y && mean && rstd && gamma && partial && coef && dy && scratch && C % 8 == 0 && C <= 2048,
@@ -711,10 +708,10 @@ extern "C" int32_t c3d_bn_bwd(const void* dout, const void* out, const void* y, 
   if (P == 0) return C3D_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int blocks = c3d_bn_bwd_blocks(P, C);
-  const long long ds = dout_stride ? dout_stride : C, os = out_stride ? out_stride : C;
+  const long long ds = dout_stride ? dout_stride : C;
   if (C / 8 <= 256)
     bn_bwd_reduce_kernel<256><<<blocks, 256, 0, st>>>((const bf16*)dout, (const bf16*)out, (const bf16*)y, mean, rstd,
-                                                       relu, partial, P, C, ds, os, gamma, beta);
+                                                       relu, partial, P, C, ds, gamma, beta);
   else
     return set_error(C3D_EINVAL, "bn_bwd: C too large");
   FinArgs A{};
@@ -724,37 +721,25 @@ extern "C" int32_t c3d_bn_bwd(const void* dout, const void* out, const void* y, 
   if (rc != C3D_OK) return rc;
   bn_bwd_apply_kernel<<<grid_for(P * (C / 8), 256), 256, 0, st>>>((const bf16*)dout, (const bf16*)out, (const bf16*)y,
                                                                    mean, rstd, coef, relu, (bf16*)dy, (bf16*)dres, P, C,
-                                                                   ds, os, dres_stride ? dres_stride : C, gamma, beta,
-                                                                   dres_acc);
+                                                                   ds, dres_stride ? dres_stride : C, gamma, beta, dres_acc);
   return check_launch("bn_bwd");
 }
-extern "C" int32_t c3d_maxpool2_fwd(const void* x, void* y, int32_t N, int32_t H, int32_t W, int32_t C,
-                                    int64_t x_stride, int64_t y_stride, void* stream) {
+extern "C" int32_t c3d_maxpool2_fwd(const void* x, void* y, int32_t N, int32_t H, int32_t W, int32_t C, void* stream) {
   C3D_REQ(x && y && C % 8 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2: bad args");
   long long work = (long long)N * (H / 2) * (W / 2) * (C / 8);
   if (work == 0) return C3D_OK;
-  maxpool2_fwd_kernel<<<grid_for(work, 256), 256, 0, (cudaStream_t)stream>>>(
-      (const bf16*)x, (bf16*)y, N, H, W, C, x_stride ? x_stride : C, y_stride ? y_stride : C);
+  maxpool2_fwd_kernel<<<grid_for(work, 256), 256, 0, (cudaStream_t)stream>>>((const bf16*)x, (bf16*)y, N, H, W, C);
   return check_launch("maxpool2_fwd");
 }
-extern "C" int32_t c3d_maxpool2_bwd(const void* x, const void* dy, void* dx, int32_t N, int32_t H, int32_t W,
-                                    int32_t C, int64_t x_stride, int64_t dy_stride, void* stream) {
+extern "C" int32_t c3d_maxpool2_bwd(const void* x, const void* dy, void* dx, int32_t N, int32_t H, int32_t W, int32_t C,
+                                    int64_t dy_stride, int64_t dx_stride, int32_t accumulate, void* stream) {
   C3D_REQ(x && dy && dx && C % 8 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2_bwd: bad args");
   long long work = (long long)N * (H / 2) * (W / 2) * (C / 8);
   if (work == 0) return C3D_OK;
-  maxpool2_bwd_kernel<false><<<grid_for(work, 256), 256, 0, (cudaStream_t)stream>>>(
-      (const bf16*)x, (const bf16*)dy, (bf16*)dx, N, H, W, C, x_stride ? x_stride : C, dy_stride ? dy_stride : C, C);
+  auto kern = accumulate ? maxpool2_bwd_kernel<true> : maxpool2_bwd_kernel<false>;
+  kern<<<grid_for(work, 256), 256, 0, (cudaStream_t)stream>>>((const bf16*)x, (const bf16*)dy, (bf16*)dx, N, H, W, C,
+                                                              dy_stride ? dy_stride : C, dx_stride ? dx_stride : C);
   return check_launch("maxpool2_bwd");
-}
-extern "C" int32_t c3d_maxpool2_bwd_acc(const void* x, const void* dy, void* dx, int32_t N, int32_t H, int32_t W,
-                                        int32_t C, int64_t x_stride, int64_t dy_stride, int64_t dx_stride, void* stream) {
-  C3D_REQ(x && dy && dx && C % 8 == 0 && H % 2 == 0 && W % 2 == 0, "maxpool2_bwd_acc: bad args");
-  long long work = (long long)N * (H / 2) * (W / 2) * (C / 8);
-  if (work == 0) return C3D_OK;
-  maxpool2_bwd_kernel<true><<<grid_for(work, 256), 256, 0, (cudaStream_t)stream>>>(
-      (const bf16*)x, (const bf16*)dy, (bf16*)dx, N, H, W, C, x_stride ? x_stride : C, dy_stride ? dy_stride : C,
-      dx_stride ? dx_stride : C);
-  return check_launch("maxpool2_bwd_acc");
 }
 extern "C" int32_t c3d_maxpool3s2_fwd(const void* x, void* y, int32_t N, int32_t H, int32_t W, int32_t C, void* stream) {
   C3D_REQ(x && y && C % 8 == 0 && H >= 1 && W >= 1, "maxpool3s2: bad args");
@@ -808,20 +793,12 @@ extern "C" int32_t c3d_grad_finite(const float* g, int64_t n, int32_t* flag, voi
   grad_finite_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(g, n, flag);
   return check_launch("grad_finite");
 }
-extern "C" int32_t c3d_sgd_momentum(float* p, const float* g, float* mom, int64_t n, float lr, float momentum,
-                                    float weight_decay, float grad_scale, const int32_t* skip_flag, void* stream) {
+extern "C" int32_t c3d_sgd_momentum(float* p, const float* g, float* mom, int64_t n, float lr, const float* lr_dev,
+                                    float momentum, float weight_decay, float grad_scale, const int32_t* skip_flag,
+                                    void* stream) {
   C3D_REQ(p && g && mom, "sgd: bad args");
   if (n == 0) return C3D_OK;
-  sgd_momentum_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(p, g, mom, n, lr, nullptr, momentum,
-                                                                           weight_decay, grad_scale, skip_flag);
-  return check_launch("sgd");
-}
-extern "C" int32_t c3d_sgd_momentum_dev(float* p, const float* g, float* mom, int64_t n, const float* lr_dev,
-                                        float momentum, float weight_decay, float grad_scale,
-                                        const int32_t* skip_flag, void* stream) {
-  C3D_REQ(p && g && mom && lr_dev, "sgd: bad args");
-  if (n == 0) return C3D_OK;
-  sgd_momentum_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(p, g, mom, n, 0.f, lr_dev, momentum,
+  sgd_momentum_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(p, g, mom, n, lr, lr_dev, momentum,
                                                                            weight_decay, grad_scale, skip_flag);
   return check_launch("sgd");
 }

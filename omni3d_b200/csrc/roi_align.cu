@@ -75,7 +75,7 @@ __device__ __forceinline__ void acc8(float (&a)[8], const bf16* p, float w) {
 // no gradient
 __device__ __forceinline__ bool roi_sane(const float* roi, const RoiLevels& L) {
   const float fb = roi[0], fl = roi[1];
-  return fb >= 0.f && (L.num_images <= 0 || fb < (float)L.num_images) && fl >= 0.f && fl < (float)L.num_levels &&
+  return fb >= 0.f && fb < (float)L.num_images && fl >= 0.f && fl < (float)L.num_levels &&
          isfinite(roi[2]) && isfinite(roi[3]) && isfinite(roi[4]) && isfinite(roi[5]);
 }
 
@@ -398,6 +398,7 @@ static int32_t run(bool bwd, const c3d_roi_levels* lv, const float* rois, int R,
                    const void* dout, cudaStream_t st) {
   if (!lv || lv->num_levels < 1 || lv->num_levels > 5 || C % 8 != 0) return set_error(C3D_EINVAL, "roi_align: bad args");
   if (R < 0) return set_error(C3D_EINVAL, "roi_align: negative R");
+  if (lv->num_images <= 0) return set_error(C3D_EINVAL, "roi_align: num_images must be set");
   RoiLevels L;
   L.num_levels = lv->num_levels;
   L.num_images = lv->num_images;
@@ -413,7 +414,6 @@ static int32_t run(bool bwd, const c3d_roi_levels* lv, const float* rois, int R,
     roi_align_kernel<<<(unsigned)blocks, 256, 0, st>>>(L, rois, R, C, PH, PW, (bf16*)out);
     return check_launch("roi_align");
   }
-  if (L.num_images <= 0) return set_error(C3D_EINVAL, "roi_align bwd: num_images must be set");
   if (PH < 1 || PW < 1 || PH > 255 || PW > 255) return set_error(C3D_EINVAL, "roi_align bwd: pooled size outside [1, 255]");
   static bool attr = false;
   if (!attr) {

@@ -10,12 +10,17 @@ from ._lib import ptr, stream
 vp, i32, f32 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_float
 
 
+def _bn_scratch(C, device):
+    """the column-sum scratch of c3d_bn_finalize / c3d_bn_bwd / c3d_bias_act_bwd, of the size the library asks for"""
+    return torch.empty(_lib.lib().c3d_bn_scratch_bytes(C), device=device, dtype=torch.uint8)
+
+
 def bn_finalize(stats, count, eps, momentum, running_mean, running_var):
     L = _lib.lib()
     rows, _, C = stats.shape
     mean = torch.empty(C, device=stats.device, dtype=torch.float32)
     rstd = torch.empty(C, device=stats.device, dtype=torch.float32)
-    scratch = torch.empty(128 * 2 * C + 64, device=stats.device, dtype=torch.float64)
+    scratch = _bn_scratch(C, stats.device)
     _lib.check(L.c3d_bn_finalize(ptr(stats), rows, C, float(count), eps, momentum, ptr(running_mean), ptr(running_var),
                                  ptr(mean), ptr(rstd), ptr(scratch), stream()), launches=1)
     return mean, rstd
@@ -28,7 +33,7 @@ def bn_apply(y, mean, rstd, gamma, beta, residual=None, relu=True, out=None):
     if out is None:
         out = torch.empty_like(y)
     _lib.check(L.c3d_bn_apply(ptr(y), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(residual), int(relu), ptr(out), P, C,
-                              0, 0, stream()))
+                              stream()))
     return out
 
 
@@ -67,9 +72,9 @@ def bn_bwd(dout, out, y, mean, rstd, gamma, relu, dgamma, dbeta, want_dres, froz
         dres, flags = dres_into, flags | 2
     else:
         dres = torch.empty_like(y) if want_dres else None
-    scratch = torch.empty(128 * 2 * C + 64, device=y.device, dtype=torch.float64)
+    scratch = _bn_scratch(C, y.device)
     _lib.check(L.c3d_bn_bwd(ptr(dout), ptr(out), ptr(y), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), flags, int(frozen), ptr(partial), ptr(coef),
-                            ptr(dgamma), ptr(dbeta), ptr(dy), ptr(dres), P, C, ds, 0, rs, ptr(scratch), stream()), launches=3)
+                            ptr(dgamma), ptr(dbeta), ptr(dy), ptr(dres), P, C, ds, rs, ptr(scratch), stream()), launches=3)
     return dy, dres
 
 
@@ -77,7 +82,7 @@ def maxpool2_fwd(x):
     L = _lib.lib()
     N, H, W, C = x.shape
     y = torch.empty((N, H // 2, W // 2, C), device=x.device, dtype=x.dtype)
-    _lib.check(L.c3d_maxpool2_fwd(ptr(x), ptr(y), N, H, W, C, 0, 0, stream()))
+    _lib.check(L.c3d_maxpool2_fwd(ptr(x), ptr(y), N, H, W, C, stream()))
     return y
 
 
@@ -88,13 +93,12 @@ def maxpool2_bwd(x, dy, into=None):
     ds = pixel_stride(dy)
     if ds is None:
         dy, ds = dy.contiguous(), 0
-    if into is not None:
-        xs = pixel_stride(into)
+    if into is None:
+        dx, xs = torch.empty_like(x), 0
+    else:
+        dx, xs = into, pixel_stride(into)
         assert xs is not None and into.dtype == torch.bfloat16
-        _lib.check(L.c3d_maxpool2_bwd_acc(ptr(x), ptr(dy), ptr(into), N, H, W, C, 0, ds, xs, stream()))
-        return into
-    dx = torch.empty_like(x)
-    _lib.check(L.c3d_maxpool2_bwd(ptr(x), ptr(dy), ptr(dx), N, H, W, C, 0, ds, stream()))
+    _lib.check(L.c3d_maxpool2_bwd(ptr(x), ptr(dy), ptr(dx), N, H, W, C, ds, xs, int(into is not None), stream()))
     return dx
 
 
@@ -186,12 +190,9 @@ def grad_finite(flat_grad, flag):
 def sgd_momentum(p, g, mom, lr, momentum, weight_decay, grad_scale=1.0, skip_flag=None):
     """lr: python float, or a 1-element fp32 CUDA tensor (read by the kernel at run time: CUDA-graph friendly)."""
     L = _lib.lib()
-    if torch.is_tensor(lr):
-        _lib.check(L.c3d_sgd_momentum_dev(ptr(p), ptr(g), ptr(mom), p.numel(), ptr(lr), momentum, weight_decay, grad_scale,
-                                          ptr(skip_flag), stream()))
-    else:
-        _lib.check(L.c3d_sgd_momentum(ptr(p), ptr(g), ptr(mom), p.numel(), lr, momentum, weight_decay, grad_scale,
-                                      ptr(skip_flag), stream()))
+    lr_dev, lr = (lr, 0.0) if torch.is_tensor(lr) else (None, lr)
+    _lib.check(L.c3d_sgd_momentum(ptr(p), ptr(g), ptr(mom), p.numel(), lr, ptr(lr_dev), momentum, weight_decay, grad_scale,
+                                  ptr(skip_flag), stream()))
 
 
 _nms_ws = {}
@@ -285,7 +286,7 @@ def bias_act_bwd(dout, out, relu, dbias):
     dout = dout.contiguous()
     blocks = L.c3d_bn_bwd_blocks(P, C)
     partial = torch.empty((blocks, C), device=dout.device, dtype=torch.float32)
-    scratch = torch.empty(128 * 2 * C + 64, device=dout.device, dtype=torch.float64)
+    scratch = _bn_scratch(C, dout.device)
     alias = (not relu) and dout.dtype == torch.bfloat16          # no activation: dz IS dout, only the bias gradient is left
     if alias and dbias is None:
         return dout

@@ -157,11 +157,17 @@ def _dgrad_chained(sink, dy, w, stride, pad, in_hw):
     return _deliver(sink, _dgrad(dy, w, stride, pad, in_hw))
 
 
+def _own_grad(p):
+    """p's own fp32 .grad (the trainer's flat arena), which a kernel can accumulate into in place, or None"""
+    g = p.grad if p.is_leaf else None
+    return g if g is not None and g.dtype == torch.float32 and g.shape == p.shape else None
+
+
 def _wgrad_to_master(x, dy, w, stride, pad):
     """weight gradient in the master (Cout,Cin,KH,KW) layout.  When the parameter already owns a contiguous
     fp32 .grad (the trainer's flat arena) the kernel accumulates straight into it and autograd gets None."""
-    g = w.grad if w.is_leaf else None
-    if g is not None and g.dtype == torch.float32 and g.shape == w.shape:
+    g = _own_grad(w)
+    if g is not None:
         if g.is_contiguous():
             K.conv2d_wgrad(x, dy, w.shape[2], w.shape[3], stride, pad, dw=g, oihw=True)
             return None
@@ -171,10 +177,19 @@ def _wgrad_to_master(x, dy, w, stride, pad):
     return K.conv2d_wgrad(x, dy, w.shape[2], w.shape[3], stride, pad, oihw=True)
 
 
+def _linear_wgrad_to_master(x, dz, w, chw, blocks=None):
+    """linear weight gradient in the master layout, accumulated straight into w's own .grad when it has one (-> None)"""
+    g = _own_grad(w)
+    if g is not None and g.is_contiguous():
+        K.linear_wgrad(x, dz, dw=g, chw=chw, blocks=blocks)
+        return None
+    return K.linear_wgrad(x, dz, chw=chw, blocks=blocks)
+
+
 def _grad_slot(p):
     """(.grad to accumulate into in place, or a fresh zero buffer; True if autograd must be given the buffer)"""
-    g = p.grad if p.is_leaf else None
-    if g is not None and g.dtype == torch.float32 and g.is_contiguous():
+    g = _own_grad(p)
+    if g is not None and g.is_contiguous():
         return g, False
     return torch.zeros_like(p, dtype=torch.float32), True
 
@@ -185,8 +200,8 @@ def _grad_slot(p):
 # per extra consumer over the whole gradient.
 # `fork(t, n)` hands every consumer its own alias of t; the aliases share a _GradSink.  The first consumer to produce
 # its gradient parks the buffer in the sink and returns it; every later consumer ADDS INTO that buffer inside the kernel
-# that produces its contribution (conv epilogue add_mode 3, c3d_bn_bwd's accumulating dres, c3d_maxpool2_bwd_acc) and
-# returns None.  _Fork.backward — which autograd runs after all consumers — folds in whatever reached it as a plain
+# that produces its contribution (conv epilogue add_mode 3, c3d_bn_bwd's accumulating dres, c3d_maxpool2_bwd's accumulate)
+# and returns None.  _Fork.backward — which autograd runs after all consumers — folds in whatever reached it as a plain
 # tensor (consumers that know nothing of sinks) and hands the buffer to the producer.  Same sums as autograd's, with
 # the adds done in fp32 before the single bf16 rounding.
 GRAD_CHAIN = True      # False: plain autograd sums (the reference the gradient-chaining tests compare against)
@@ -387,21 +402,15 @@ class LinearAct(torch.autograd.Function):
         dbias, ret_b = _grad_slot(bias) if bias is not None and ctx.needs_input_grad[2] else (None, False)
         dz = Kx.bias_act_bwd(dy, y, relu, dbias)                       # bf16 (rows, N); dbias += column sums
         dx = K.linear_dgrad(dz, wt) if ctx.needs_input_grad[0] else None
-        dw = None
-        if ctx.needs_input_grad[1]:
-            g = w.grad if w.is_leaf else None
-            if g is not None and g.dtype == torch.float32 and g.shape == w.shape and g.is_contiguous():
-                K.linear_wgrad(x, dz, dw=g, chw=chw)        # straight into the trainer's gradient arena (master layout)
-            else:
-                dw = K.linear_wgrad(x, dz, chw=chw)
+        dw = _linear_wgrad_to_master(x, dz, w, chw) if ctx.needs_input_grad[1] else None
         return dx, dw, dbias if ret_b else None, None, None, None
 
 
 class TwoHeadFC1(torch.autograd.Function):
     """First FC layer of the box head over all B*S pooled RoIs and of the cube head over the first Fc RoIs of every image
     (Base.yaml:66-68,78-80: same pooler => the cube head's RoIs are a prefix of the box head's sampled RoIs), sharing ONE
-    pooled tensor: the cube GEMM reads its rows in place (c3d_linear_fwd_blocks) and its data gradient is accumulated into
-    the box head's (c3d_linear_dgrad_blocks, in-place epilogue) — no gather copy forward, no zero-padded scatter + add
+    pooled tensor: the cube GEMM reads its rows in place (c3d_linear_fwd over row blocks) and its data gradient is accumulated
+    into the box head's (c3d_linear_dgrad, in-place epilogue) — no gather copy forward, no zero-padded scatter + add
     backward (~1 GB of HBM traffic per step at batch 32)."""
 
     @staticmethod
@@ -410,7 +419,7 @@ class TwoHeadFC1(torch.autograd.Function):
         wpb, wtb = _packed_linear(wb, chw)
         wpc, wtc = _packed_linear(wc, chw)
         hb = K.linear_fwd(x, wpb, bb.detach().float().contiguous(), relu=True)
-        hc = K.linear_fwd_blocks(x, B, Fc, S, wpc, bc.detach().float().contiguous(), relu=True)
+        hc = K.linear_fwd(x, wpc, bc.detach().float().contiguous(), relu=True, blocks=(B, Fc, S))
         ctx.save_for_backward(x, wb, bb, wc, bc, hb, hc, wtb, wtc)
         ctx.cfg = (B, S, Fc, chw)
         return hb, hc
@@ -430,16 +439,9 @@ class TwoHeadFC1(torch.autograd.Function):
         dx = None
         if ctx.needs_input_grad[0]:
             dx = K.linear_dgrad(dzb, wtb)
-            K.linear_dgrad_blocks(dzc, wtc, dx, B, Fc, S, accumulate=True)
-
-        def wgrad(w, fn):
-            g = w.grad if w.is_leaf else None
-            if g is not None and g.dtype == torch.float32 and g.shape == w.shape and g.is_contiguous():
-                fn(g)
-                return None
-            return fn(None)
-        dwb = wgrad(wb, lambda g: K.linear_wgrad(x, dzb, dw=g, chw=chw))
-        dwc = wgrad(wc, lambda g: K.linear_wgrad_blocks(x, dzc, B, Fc, S, dw=g, chw=chw))
+            K.linear_dgrad(dzc, wtc, blocks=(B, Fc, S), dx=dx, accumulate=True)
+        dwb = _linear_wgrad_to_master(x, dzb, wb, chw)
+        dwc = _linear_wgrad_to_master(x, dzc, wc, chw, blocks=(B, Fc, S))
         return dx, dwb, gbb if rb else None, dwc, gbc if rc else None, None, None, None, None
 
 

@@ -193,3 +193,31 @@ def test_conv_descriptor_argument_checks_without_gpu():
     assert call(desc(stride=3), addend=None) == _lib.C3D_EINVAL and b"stride" in L.c3d_last_error()
     with pytest.raises(_lib.C3DError):
         _lib.check(_lib.C3D_EINVAL)
+
+
+def test_entry_point_argument_checks_without_gpu():
+    """the linear, weight-gradient, SGD, max-pool backward, linear-weight pack and ROIAlign entry points reject bad
+    arguments with C3D_EINVAL and a message before any CUDA call; an empty linear layer is a no-op."""
+    from omni3d_b200 import _lib
+    L = _lib.lib()
+    p = ctypes.c_void_p(256)                       # non-null dummies: every case below is rejected before they are used
+
+    def einval(rc, msg):
+        return rc == _lib.C3D_EINVAL and msg in L.c3d_last_error()
+
+    # linear layers: (nseg, seg_rows, seg_stride) row blocks
+    assert einval(L.c3d_linear_fwd(p, p, None, p, 2, 64, 32, 64, 64, 0, 0, None), b"seg_stride < seg_rows")
+    assert einval(L.c3d_linear_dgrad(p, p, p, 2, 64, 63, 64, 64, 1, None), b"seg_stride < seg_rows")
+    assert einval(L.c3d_linear_wgrad(p, p, p, 1, 2**31, 2**31, 64, 64, 0, 0, None), b"INT32_MAX")   # no silent truncation
+    assert einval(L.c3d_linear_fwd(p, p, None, p, 1, 2**31, 2**31, 64, 64, 0, 0, None), b"INT32_MAX")
+    assert L.c3d_linear_fwd(p, p, None, p, 0, 64, 64, 64, 64, 0, 0, None) == _lib.C3D_OK                # nothing to do
+    assert L.c3d_linear_dgrad(p, p, p, 4, 0, 0, 64, 64, 0, None) == _lib.C3D_OK
+    d = _lib.ConvDesc(N=2, H=8, W=8, Cin=64, Cout=64, KH=3, KW=3, stride=1, pad=1)
+    assert einval(L.c3d_conv2d_wgrad(ctypes.byref(d), p, p, None, 1, None), b"wgrad: null pointer")
+    assert einval(L.c3d_sgd_momentum(None, p, p, 1024, 0.1, None, 0.9, 1e-4, 1.0, None, None), b"sgd")
+    assert einval(L.c3d_maxpool2_bwd(p, p, p, 2, 8, 8, 12, 0, 0, 1, None), b"maxpool2_bwd")             # C % 8 != 0
+    assert einval(L.c3d_pack_linear_weight(p, 64, 64, 0, 0, p, None, None), b"pack_linear_weight")      # no transpose
+    lv = _lib.RoiLevels(num_levels=1, num_images=0)
+    lv.feat[0], lv.H[0], lv.W[0], lv.scale[0] = 256, 8, 8, 0.25
+    assert einval(L.c3d_roi_align_fwd(ctypes.byref(lv), p, 4, 64, 7, 7, p, None), b"num_images")
+    assert einval(L.c3d_roi_align_bwd(ctypes.byref(lv), p, 4, 64, 7, 7, p, None), b"num_images")
