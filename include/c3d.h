@@ -276,17 +276,21 @@ int32_t c3d_clip_grad(float* g, int64_t n, int32_t mode, float clip_value, float
 /* ------------------------------------------------------------------------------------------
  * Multi-level ROIAlign (aligned=True, sampling_ratio 0) on NHWC bf16 FPN maps.
  * Replaces detectron2 ROIPooler/ROIAlignV2 at cubercnn/modeling/roi_heads/roi_heads.py:267,362.
- * rois: fp32 [R][6] = (batch index, level index, x1, y1, x2, y2).  out: bf16 [R][ph][pw][C].
+ * rois: fp32 [R][6] = (batch index, level index, x1, y1, x2, y2).  out: bf16 [R][ph][pw][C].  C must be a multiple of 8;
+ * the backward reads dout (bf16 [R][ph][pw][C]) 16 bytes at a time, so dout must be 16-byte aligned (EINVAL otherwise).
  * RoIs with a non-finite coordinate, a level outside [0, num_levels) or an image index outside [0, num_images) pool
  * zeros / contribute no gradient instead of indexing out of bounds.
  * ------------------------------------------------------------------------------------------ */
 typedef struct {
   const void* feat[5];   /* level l: bf16 (N,H[l],W[l],C) */
-  void* grad[5];         /* backward only: fp32 (N,H[l],W[l],C), written (every element, in one fixed order) */
+  void* grad[5];         /* backward only: (N,H[l],W[l],C) fp32 or bf16 (grad_bf16), written (every element, in one
+                            fixed order) */
   int32_t H[5], W[5];
   float scale[5];
   int32_t num_levels;
   int32_t num_images;    /* N of the maps (> 0) */
+  int32_t grad_bf16;     /* backward only: 0 writes fp32 maps, 1 writes bf16 maps, each element the fp32 sum rounded once
+                            to nearest even (what casting the fp32 map to bf16 gives for every finite value) */
 } c3d_roi_levels;
 int32_t c3d_roi_align_fwd(const c3d_roi_levels* levels, const float* rois, int32_t R, int32_t C, int32_t pooled_h,
                           int32_t pooled_w, void* out, void* stream);

@@ -37,7 +37,7 @@ class PackDesc(ctypes.Structure):
 
 class RoiLevels(ctypes.Structure):
     _fields_ = [("feat", vp * 5), ("grad", vp * 5), ("H", i32 * 5), ("W", i32 * 5), ("scale", f32 * 5),
-                ("num_levels", i32), ("num_images", i32)]
+                ("num_levels", i32), ("num_images", i32), ("grad_bf16", i32)]
 
 
 class TopkSeg(ctypes.Structure):

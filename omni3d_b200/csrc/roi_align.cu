@@ -11,6 +11,7 @@
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include "c3d_common.cuh"
+#include "roi_geom.cuh"
 
 namespace c3d {
 using bf16 = __nv_bfloat16;
@@ -22,47 +23,8 @@ struct RoiLevels {
   float scale[5];
   int num_levels;
   int num_images;
+  int grad_bf16;
 };
-
-// Sample geometry, shared by the forward and the backward so that both round alike.  Each operation is written out
-// (fmaf, __fadd_rn, __fmul_rn, __fdiv_rn) as the forward has always compiled it, so no contraction the compiler might
-// choose differently in one kernel can change a weight.
-struct RoiGeom { float sw, sh, rw, rh, bw, bh, cnt; int gw, gh; };
-
-__device__ __forceinline__ RoiGeom roi_geom(const float* roi, float sc, int PH, int PW) {
-  RoiGeom g;
-  g.sw = fmaf(roi[2], sc, -0.5f);
-  g.sh = fmaf(roi[3], sc, -0.5f);
-  g.rw = __fsub_rn(fmaf(roi[4], sc, -0.5f), g.sw);
-  g.rh = __fsub_rn(fmaf(roi[5], sc, -0.5f), g.sh);
-  g.bw = __fdiv_rn(g.rw, (float)PW);
-  g.bh = __fdiv_rn(g.rh, (float)PH);
-  g.gw = (int)ceilf(g.bw);
-  g.gh = (int)ceilf(g.bh);
-  g.cnt = fmaxf((float)(g.gh * g.gw), 1.f);
-  return g;
-}
-
-// coordinate of sample i of n in bin p of size b that starts the RoI at s: s + p * b + (i + 0.5) * b / n
-__device__ __forceinline__ float sample_at(float s, int p, float b, int i, int n) {
-  return __fadd_rn(fmaf((float)p, b, s), __fdiv_rn(__fmul_rn(__fadd_rn((float)i, 0.5f), b), (float)n));
-}
-
-struct Tap { int y0, y1, x0, x1; float w1, w2, w3, w4; bool valid; };
-
-__device__ __forceinline__ Tap make_tap(float y, float x, int H, int W) {
-  Tap t;
-  t.valid = !(y < -1.0f || y > (float)H || x < -1.0f || x > (float)W);
-  if (y <= 0.f) y = 0.f;
-  if (x <= 0.f) x = 0.f;
-  int yl = (int)y, xl = (int)x, yh, xh;
-  if (yl >= H - 1) { yh = yl = H - 1; y = (float)yl; } else yh = yl + 1;
-  if (xl >= W - 1) { xh = xl = W - 1; x = (float)xl; } else xh = xl + 1;
-  const float ly = __fsub_rn(y, (float)yl), lx = __fsub_rn(x, (float)xl), hy = __fsub_rn(1.f, ly), hx = __fsub_rn(1.f, lx);
-  t.y0 = yl; t.y1 = yh; t.x0 = xl; t.x1 = xh;
-  t.w1 = __fmul_rn(hy, hx); t.w2 = __fmul_rn(hy, lx); t.w3 = __fmul_rn(ly, hx); t.w4 = __fmul_rn(ly, lx);
-  return t;
-}
 
 __device__ __forceinline__ void acc8(float (&a)[8], const bf16* p, float w) {
   uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
@@ -71,12 +33,8 @@ __device__ __forceinline__ void acc8(float (&a)[8], const bf16* p, float w) {
   for (int i = 0; i < 4; ++i) { float2 f = __bfloat1622float2(h[i]); a[2 * i] += w * f.x; a[2 * i + 1] += w * f.y; }
 }
 
-// a NaN / Inf box (diverging step) must not become an out-of-range level or image index: such RoIs pool zeros and get
-// no gradient
 __device__ __forceinline__ bool roi_sane(const float* roi, const RoiLevels& L) {
-  const float fb = roi[0], fl = roi[1];
-  return fb >= 0.f && fb < (float)L.num_images && fl >= 0.f && fl < (float)L.num_levels &&
-         isfinite(roi[2]) && isfinite(roi[3]) && isfinite(roi[4]) && isfinite(roi[5]);
+  return roi_in_range(roi, L.num_images, L.num_levels);
 }
 
 // rois: [R][6] = (batch, level, x1, y1, x2, y2) fp32
@@ -124,21 +82,19 @@ __global__ void roi_align_kernel(RoiLevels L, const float* __restrict__ rois, in
 // ------------------------------------------------------------------------------------------------------------------
 // Backward: a gather with no atomics, in two launches.
 //
-// roi_bucket_kernel lists the RoI indices of every (image, level) in index order (a stable counting sort).
+// roi_bucket_kernel lists the RoI indices of every (image, level) in index order (a stable counting sort), and with each
+// one the rows and columns its bins can reach (a conservative rectangle, computed once per RoI).
 //
-// roi_align_bwd_kernel: grid = (sum over levels of ceil(H / 8) bands, images).  A block owns one (image, level, 8-row
-// band) of the gradient map and walks the band's 8 x 8 pixel tiles.  For a tile it reads its bucket 256 RoIs at a time
-// and lists the bins of those RoIs that can reach the tile, as "slots" (kSlots at a time, in (RoI, ph, pw) order).
-// The threads then split the (slot, iy, ix) samples among themselves; each computes its sample's four taps once and
-// keeps those that fall in the tile as (pixel, slot, weight) entries, compacted in (sample, tap) order.  Thread t owns
-// channel cc + t: it stages g = dout / count of every slot for its channel and walks the entries, adding w * g to its
+// roi_align_bwd_kernel: grid = (sum over levels of the 8 x 8 pixel tiles of a map, images).  A block owns one tile of
+// one (image, level) gradient map.  It reads the bucket 256 RoIs at a time, drops those whose rectangle misses the tile,
+// and lists the bins of the rest that can reach the tile, as "slots" (kSlots at a time, in (RoI, ph, pw) order).  The
+// threads stage g = dout / count of every slot (16 bytes of dout per load) and split the (slot, iy, ix) samples among
+// themselves; each computes its sample's four taps once and keeps those that fall in the tile as (pixel, slot, weight)
+// entries, compacted in (sample, tap) order.  Thread t owns channel cc + t and walks the entries, adding w * g to its
 // column of a [64 px][256 ch] fp32 tile in shared memory.  Every element of the map thus receives
 // acc = fmaf(w, g, acc), starting from +0, over (RoI, ph, pw, iy, ix, tap) in that order, as one chain, and is stored
-// once, zeros included: the maps need no clearing.  Storing the chain is the same as adding it to a zeroed map, since
-// the chain is never -0.
-// (Up to version 2 of the ABI the kernel added to the map and split a band's RoIs into lists of 2048, adding each list's
-// sum separately; results can differ from that only where more than 2048 RoIs of one image and level reach one band.
-// Training samples at most 512 RoIs per image.)
+// once, zeros included, as fp32 or rounded once to bf16: the maps need no clearing.  Storing the chain is the same as
+// adding it to a zeroed map, since the chain is never -0.
 constexpr int kTile = 8, kTileC = 256, kSlots = 32, kEntCap = 4 * kTileC;
 constexpr int kBucketThreads = 1024, kBucketWarps = kBucketThreads / 32;
 
@@ -185,12 +141,25 @@ __device__ __forceinline__ int roi_bucket(const float* roi, const RoiLevels& L) 
   return roi_sane(roi, L) ? (int)roi[0] * L.num_levels + (int)roi[1] : -1;
 }
 
+// Rows [x, y] and columns [z, w] of the map that the bins of a RoI can reach, as the tile kernel tests its bins: bin ph
+// is kept for tile rows [t0, t1] when floor(sh + ph * bh) - 1 <= t1 and floor(sh + (ph + 1) * bh) + 1 >= t0.  Those
+// bounds grow with ph, so every kept bin lies within floor(sh) - 1 and floor(sh + PH * bh) + 1; one more row on the far
+// side covers a different rounding of sh + PH * bh.  Floats, so that no bound of a huge box overflows an int.  A RoI
+// with no samples gets an empty rectangle.
+__device__ __forceinline__ float4 roi_reach(const float* roi, float sc, int PH, int PW) {
+  const RoiGeom g = roi_geom(roi, sc, PH, PW);
+  if (g.gh <= 0 || g.gw <= 0) return make_float4(INFINITY, -INFINITY, INFINITY, -INFINITY);
+  return make_float4(floorf(g.sh) - 1.f, floorf(fmaf((float)PH, g.bh, g.sh)) + 2.f,
+                     floorf(g.sw) - 1.f, floorf(fmaf((float)PW, g.bw, g.sw)) + 2.f);
+}
+
 // One block.  Warp w takes the w-th contiguous slice of [0, R) and counts its keys into wk[w][key]; the counts become
 // start offsets (bucket by bucket, and warp by warp inside a bucket), and a second pass places every index.
-// wk: kBucketWarps x nb ints of scratch; off: nb + 1 bucket offsets; idx: the bucketed RoI indices.
+// wk: kBucketWarps x nb ints of scratch; off: nb + 1 bucket offsets; idx: the bucketed RoI indices; reach: their
+// roi_reach rectangles, in the same order.
 __global__ void __launch_bounds__(kBucketThreads)
-roi_bucket_kernel(RoiLevels L, const float* __restrict__ rois, int R, int nb, int* __restrict__ wk, int* __restrict__ off,
-                  int* __restrict__ idx) {
+roi_bucket_kernel(RoiLevels L, const float* __restrict__ rois, int R, int nb, int PH, int PW, int* __restrict__ wk,
+                  int* __restrict__ off, int* __restrict__ idx, float4* __restrict__ reach) {
   __shared__ int s_part[kBucketWarps];
   __shared__ int s_carry;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -241,7 +210,12 @@ roi_bucket_kernel(RoiLevels L, const float* __restrict__ rois, int R, int nb, in
     int base = 0;
     if (k >= 0 && lane == leader) base = atomicAdd(&mine[k], __popc(peers));
     base = __shfl_sync(0xffffffffu, base, leader);
-    if (k >= 0) idx[base + __popc(peers & ((1u << lane) - 1u))] = r;
+    if (k >= 0) {
+      const int at = base + __popc(peers & ((1u << lane) - 1u));
+      const float* roi = rois + (size_t)r * 6;
+      idx[at] = r;
+      reach[at] = roi_reach(roi, L.scale[(int)roi[1]], PH, PW);
+    }
   }
 }
 
@@ -256,33 +230,41 @@ __device__ __forceinline__ void sample_range(float s, float st, int n, int t0, i
   count = max(0, last - first + 1);
 }
 
+__device__ __forceinline__ void store_grad(float* p, float v) { *p = v; }
+__device__ __forceinline__ void store_grad(bf16* p, float v) { *p = __float2bfloat16_rn(v); }
+
+template <typename OutT>
 __global__ void __launch_bounds__(kTileC, 2)
 roi_align_bwd_kernel(RoiLevels L, const float* __restrict__ rois, const int* __restrict__ off, const int* __restrict__ idx,
-                     int C, int PH, int PW, const bf16* __restrict__ dout) {
+                     const float4* __restrict__ reach, int C, int PH, int PW, const bf16* __restrict__ dout) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   BwdSmem& S = *reinterpret_cast<BwdSmem*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31;
   const int b = blockIdx.y;
-  int lvl = 0, band = blockIdx.x;
-  while (lvl < L.num_levels - 1 && band >= (L.H[lvl] + kTile - 1) / kTile) { band -= (L.H[lvl] + kTile - 1) / kTile; ++lvl; }
+  int lvl = 0, tile = blockIdx.x;
+  auto tiles_of = [&](int l) { return ((L.H[l] + kTile - 1) / kTile) * ((L.W[l] + kTile - 1) / kTile); };
+  while (lvl < L.num_levels - 1 && tile >= tiles_of(lvl)) { tile -= tiles_of(lvl); ++lvl; }
+  if (tile >= tiles_of(lvl)) return;
   const int H = L.H[lvl], W = L.W[lvl];
-  if (band * kTile >= H) return;
   const float sc = L.scale[lvl];
-  const int ty0 = band * kTile, ty1 = min(H, ty0 + kTile) - 1;
+  const int ntx = (W + kTile - 1) / kTile;
+  const int ty0 = tile / ntx * kTile, ty1 = min(H, ty0 + kTile) - 1;
+  const int tx0 = tile % ntx * kTile, tx1 = min(W, tx0 + kTile) - 1;
   const int key = b * L.num_levels + lvl;
   const int* list = idx + off[key];
+  const float4* lreach = reach + off[key];
   const int n = off[key + 1] - off[key];
-  float* gmap = L.grad[lvl] + (size_t)b * H * W * C;
-  for (int tx0 = 0; tx0 < W; tx0 += kTile) {
-    const int tx1 = min(W, tx0 + kTile) - 1;
-    for (int cc = 0; cc < C; cc += kTileC) {
-      const int c = cc + tid;
+  OutT* gmap = reinterpret_cast<OutT*>(L.grad[lvl]) + (size_t)b * H * W * C;
+  for (int cc = 0; cc < C; cc += kTileC) {
+    const int c = cc + tid;
 #pragma unroll 8
-      for (int p = 0; p < kTile * kTile; ++p) S.acc[p][tid] = 0.f;
-      for (int w0 = 0; w0 < n; w0 += kTileC) {
-        // ---- the bins of the next kTileC RoIs whose footprint, one pixel wider, overlaps the tile
-        int nbin = 0, rect = 0, ri = 0;
-        if (w0 + tid < n) {
+    for (int p = 0; p < kTile * kTile; ++p) S.acc[p][tid] = 0.f;
+    for (int w0 = 0; w0 < n; w0 += kTileC) {
+      // ---- the bins of the next kTileC RoIs whose footprint, one pixel wider, overlaps the tile
+      int nbin = 0, rect = 0, ri = 0;
+      if (w0 + tid < n) {
+        const float4 rc = lreach[w0 + tid];
+        if (rc.x <= (float)ty1 && rc.y >= (float)ty0 && rc.z <= (float)tx1 && rc.w >= (float)tx0) {
           ri = list[w0 + tid];
           const RoiGeom g = roi_geom(rois + (size_t)ri * 6, sc, PH, PW);
           if (g.gh > 0 && g.gw > 0) {
@@ -303,94 +285,116 @@ roi_align_bwd_kernel(RoiLevels L, const float* __restrict__ rois, const int* __r
             }
           }
         }
-        int nbins;
-        const int first = block_exclusive_scan(nbin, S.warp, nbins);
-        S.roi[tid] = ri;
-        S.rect[tid] = rect;
-        S.bins[tid] = first;
-        if (tid == 0) S.bins[kTileC] = nbins;
-        __syncthreads();
-        for (int s0 = 0; s0 < nbins; s0 += kSlots) {
-          const int ns = min(kSlots, nbins - s0);
-          // ---- slot setup, one lane per slot: which RoI and bin, and which of its samples can reach the tile
-          if (tid < 32) {
-            int items = 0;
-            if (lane < ns) {
-              const int bin = s0 + lane;
-              int lo = 0, hi = kTileC;                         // the last window RoI whose bins start at or before `bin`
-              while (hi - lo > 1) {
-                const int mid = (lo + hi) >> 1;
-                if (S.bins[mid] <= bin) lo = mid; else hi = mid;
-              }
-              const int rc = S.rect[lo], r = S.roi[lo], local = bin - S.bins[lo], npw = rc >> 16;
-              const int ph = (rc & 255) + local / npw, pw = ((rc >> 8) & 255) + local % npw;
-              const RoiGeom g = roi_geom(rois + (size_t)r * 6, sc, PH, PW);
-              int iy0, niy, ix0, nix;
-              sample_range(fmaf((float)ph, g.bh, g.sh), __fdiv_rn(g.bh, (float)g.gh), g.gh, ty0, ty1, iy0, niy);
-              sample_range(fmaf((float)pw, g.bw, g.sw), __fdiv_rn(g.bw, (float)g.gw), g.gw, tx0, tx1, ix0, nix);
-              S.sh[lane] = g.sh; S.sw[lane] = g.sw; S.bh[lane] = g.bh; S.bw[lane] = g.bw; S.cnt[lane] = g.cnt;
-              S.gh[lane] = g.gh; S.gw[lane] = g.gw; S.ph[lane] = ph; S.pw[lane] = pw; S.ri[lane] = r;
-              S.iy[lane] = iy0; S.ix[lane] = ix0; S.nix[lane] = nix;
-              items = niy * nix;
-            }
-            S.items[lane + 1] = warp_inclusive_scan(items, lane);
-            if (lane == 0) S.items[0] = 0;
-          }
-          __syncthreads();
-          // ---- g = dout / count of every slot, for this thread's channel
-          for (int s = 0; s < ns; ++s)
-            S.g[s][tid] = c < C ? __fdiv_rn(__bfloat162float(dout[(((size_t)S.ri[s] * PH + S.ph[s]) * PW + S.pw[s]) * C + c]), S.cnt[s])
-                                : 0.f;
-          const int nitems = S.items[ns];
-          for (int i0 = 0; i0 < nitems; i0 += kTileC) {
-            // ---- one sample per thread: its taps that fall in the tile, compacted in (sample, tap) order
-            const int k = i0 + tid;
-            unsigned mask = 0;
-            int slot = 0;
-            Tap t = {};
-            if (k < nitems) {
-              int lo = 0, hi = ns;
-              while (hi - lo > 1) {
-                const int mid = (lo + hi) >> 1;
-                if (S.items[mid] <= k) lo = mid; else hi = mid;
-              }
-              slot = lo;
-              const int local = k - S.items[slot], nx = S.nix[slot];
-              const float y = sample_at(S.sh[slot], S.ph[slot], S.bh[slot], S.iy[slot] + local / nx, S.gh[slot]);
-              const float x = sample_at(S.sw[slot], S.pw[slot], S.bw[slot], S.ix[slot] + local % nx, S.gw[slot]);
-              t = make_tap(y, x, H, W);
-              if (t.valid) {
-                const bool r0 = t.y0 >= ty0 && t.y0 <= ty1, r1 = t.y1 >= ty0 && t.y1 <= ty1;
-                const bool c0 = t.x0 >= tx0 && t.x0 <= tx1, c1 = t.x1 >= tx0 && t.x1 <= tx1;
-                mask = (r0 && c0) | (r0 && c1) << 1 | (r1 && c0) << 2 | (r1 && c1) << 3;
-              }
-            }
-            int nent;
-            int q = block_exclusive_scan(__popc(mask), S.warp, nent);
-            const int tag = slot << 6;
-            if (mask & 1) S.ent[q++] = make_int2(tag | (t.y0 - ty0) * kTile + (t.x0 - tx0), __float_as_int(t.w1));
-            if (mask & 2) S.ent[q++] = make_int2(tag | (t.y0 - ty0) * kTile + (t.x1 - tx0), __float_as_int(t.w2));
-            if (mask & 4) S.ent[q++] = make_int2(tag | (t.y1 - ty0) * kTile + (t.x0 - tx0), __float_as_int(t.w3));
-            if (mask & 8) S.ent[q] = make_int2(tag | (t.y1 - ty0) * kTile + (t.x1 - tx0), __float_as_int(t.w4));
-            __syncthreads();
-            // ---- this thread's channel, entry by entry
-            for (int e = 0; e < nent; ++e) {
-              const int2 en = S.ent[e];
-              float& a = S.acc[en.x & 63][tid];
-              a = fmaf(__int_as_float(en.y), S.g[en.x >> 6][tid], a);
-            }
-            __syncthreads();
-          }
-          __syncthreads();
-        }
       }
-      if (c < C) {
-        for (int p = 0; p < kTile * kTile; ++p) {
-          const int py = ty0 + p / kTile, px = tx0 + p % kTile;
-          if (py <= ty1 && px <= tx1) gmap[((size_t)py * W + px) * C + c] = S.acc[p][tid];
+      int nbins;
+      const int first = block_exclusive_scan(nbin, S.warp, nbins);
+      if (nbins == 0) {            // uniform: no RoI of this window reaches the tile
+        __syncthreads();
+        continue;
+      }
+      S.roi[tid] = ri;
+      S.rect[tid] = rect;
+      S.bins[tid] = first;
+      if (tid == 0) S.bins[kTileC] = nbins;
+      __syncthreads();
+      for (int s0 = 0; s0 < nbins; s0 += kSlots) {
+        const int ns = min(kSlots, nbins - s0);
+        // ---- slot setup, one lane per slot: which RoI and bin, and which of its samples can reach the tile
+        if (tid < 32) {
+          int items = 0;
+          if (lane < ns) {
+            const int bin = s0 + lane;
+            int lo = 0, hi = kTileC;                         // the last window RoI whose bins start at or before `bin`
+            while (hi - lo > 1) {
+              const int mid = (lo + hi) >> 1;
+              if (S.bins[mid] <= bin) lo = mid; else hi = mid;
+            }
+            const int rc = S.rect[lo], r = S.roi[lo], local = bin - S.bins[lo], npw = rc >> 16;
+            const int ph = (rc & 255) + local / npw, pw = ((rc >> 8) & 255) + local % npw;
+            const RoiGeom g = roi_geom(rois + (size_t)r * 6, sc, PH, PW);
+            int iy0, niy, ix0, nix;
+            sample_range(fmaf((float)ph, g.bh, g.sh), __fdiv_rn(g.bh, (float)g.gh), g.gh, ty0, ty1, iy0, niy);
+            sample_range(fmaf((float)pw, g.bw, g.sw), __fdiv_rn(g.bw, (float)g.gw), g.gw, tx0, tx1, ix0, nix);
+            S.sh[lane] = g.sh; S.sw[lane] = g.sw; S.bh[lane] = g.bh; S.bw[lane] = g.bw; S.cnt[lane] = g.cnt;
+            S.gh[lane] = g.gh; S.gw[lane] = g.gw; S.ph[lane] = ph; S.pw[lane] = pw; S.ri[lane] = r;
+            S.iy[lane] = iy0; S.ix[lane] = ix0; S.nix[lane] = nix;
+            items = niy * nix;
+          }
+          S.items[lane + 1] = warp_inclusive_scan(items, lane);
+          if (lane == 0) S.items[0] = 0;
         }
+        __syncthreads();
+        // ---- g = dout / count of every slot: 8 channels per load, the slots spread over all threads.  x / 1 == x, so
+        // the common single-sample bin skips the division.
+        for (int j = tid; j < ns * (kTileC / 8); j += kTileC) {
+          const int s = j / (kTileC / 8), q = j % (kTileC / 8) * 8;
+          float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+          if (cc + q < C) {
+            const uint4 u = __ldg(reinterpret_cast<const uint4*>(
+                dout + (((size_t)S.ri[s] * PH + S.ph[s]) * PW + S.pw[s]) * C + cc + q));
+            const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) { const float2 f = __bfloat1622float2(h[i]); v[2 * i] = f.x; v[2 * i + 1] = f.y; }
+            const float cnt = S.cnt[s];
+            if (cnt != 1.f) {
+#pragma unroll
+              for (int i = 0; i < 8; ++i) v[i] = __fdiv_rn(v[i], cnt);
+            }
+          }
+          float4* dst = reinterpret_cast<float4*>(&S.g[s][q]);
+          dst[0] = make_float4(v[0], v[1], v[2], v[3]);
+          dst[1] = make_float4(v[4], v[5], v[6], v[7]);
+        }
+        const int nitems = S.items[ns];
+        for (int i0 = 0; i0 < nitems; i0 += kTileC) {
+          // ---- one sample per thread: its taps that fall in the tile, compacted in (sample, tap) order
+          const int k = i0 + tid;
+          unsigned mask = 0;
+          int slot = 0;
+          Tap t = {};
+          if (k < nitems) {
+            int lo = 0, hi = ns;
+            while (hi - lo > 1) {
+              const int mid = (lo + hi) >> 1;
+              if (S.items[mid] <= k) lo = mid; else hi = mid;
+            }
+            slot = lo;
+            const int local = k - S.items[slot], nx = S.nix[slot];
+            const float y = sample_at(S.sh[slot], S.ph[slot], S.bh[slot], S.iy[slot] + local / nx, S.gh[slot]);
+            const float x = sample_at(S.sw[slot], S.pw[slot], S.bw[slot], S.ix[slot] + local % nx, S.gw[slot]);
+            t = make_tap(y, x, H, W);
+            if (t.valid) {
+              const bool r0 = t.y0 >= ty0 && t.y0 <= ty1, r1 = t.y1 >= ty0 && t.y1 <= ty1;
+              const bool c0 = t.x0 >= tx0 && t.x0 <= tx1, c1 = t.x1 >= tx0 && t.x1 <= tx1;
+              mask = (r0 && c0) | (r0 && c1) << 1 | (r1 && c0) << 2 | (r1 && c1) << 3;
+            }
+          }
+          int nent;
+          int q = block_exclusive_scan(__popc(mask), S.warp, nent);
+          const int tag = slot << 6;
+          if (mask & 1) S.ent[q++] = make_int2(tag | (t.y0 - ty0) * kTile + (t.x0 - tx0), __float_as_int(t.w1));
+          if (mask & 2) S.ent[q++] = make_int2(tag | (t.y0 - ty0) * kTile + (t.x1 - tx0), __float_as_int(t.w2));
+          if (mask & 4) S.ent[q++] = make_int2(tag | (t.y1 - ty0) * kTile + (t.x0 - tx0), __float_as_int(t.w3));
+          if (mask & 8) S.ent[q] = make_int2(tag | (t.y1 - ty0) * kTile + (t.x1 - tx0), __float_as_int(t.w4));
+          __syncthreads();
+          // ---- this thread's channel, entry by entry
+          for (int e = 0; e < nent; ++e) {
+            const int2 en = S.ent[e];
+            float& a = S.acc[en.x & 63][tid];
+            a = fmaf(__int_as_float(en.y), S.g[en.x >> 6][tid], a);
+          }
+          __syncthreads();
+        }
+        __syncthreads();
       }
     }
+    if (c < C) {
+      for (int p = 0; p < kTile * kTile; ++p) {
+        const int py = ty0 + p / kTile, px = tx0 + p % kTile;
+        if (py <= ty1 && px <= tx1) store_grad(gmap + ((size_t)py * W + px) * C + c, S.acc[p][tid]);
+      }
+    }
+    __syncthreads();
   }
 }
 
@@ -406,6 +410,7 @@ static int32_t run(bool bwd, const c3d_roi_levels* lv, const float* rois, int R,
     L.feat[i] = (const bf16*)lv->feat[i]; L.grad[i] = (float*)lv->grad[i];
     L.H[i] = lv->H[i]; L.W[i] = lv->W[i]; L.scale[i] = lv->scale[i];
   }
+  L.grad_bf16 = lv->grad_bf16;
   if (!bwd) {
     if (R == 0) return C3D_OK;
     long long nbins = (long long)R * PH * PW;
@@ -415,29 +420,36 @@ static int32_t run(bool bwd, const c3d_roi_levels* lv, const float* rois, int R,
     return check_launch("roi_align");
   }
   if (PH < 1 || PW < 1 || PH > 255 || PW > 255) return set_error(C3D_EINVAL, "roi_align bwd: pooled size outside [1, 255]");
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(roi_align_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BwdSmem));
+  if (L.grad_bf16 != 0 && L.grad_bf16 != 1) return set_error(C3D_EINVAL, "roi_align bwd: grad_bf16 must be 0 or 1");
+  if (R > 0 && reinterpret_cast<uintptr_t>(dout) % 16 != 0)
+    return set_error(C3D_EINVAL, "roi_align bwd: dout must be 16-byte aligned");
+  auto* kernel = L.grad_bf16 ? roi_align_bwd_kernel<bf16> : roi_align_bwd_kernel<float>;
+  static bool attr[2] = {false, false};
+  if (!attr[L.grad_bf16]) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BwdSmem));
     if (e != cudaSuccess) return set_error(C3D_ECUDA, "roi_align bwd smem attr: %s", cudaGetErrorString(e));
-    attr = true;
+    attr[L.grad_bf16] = true;
   }
-  // the RoI buckets live in stream-ordered scratch: offsets (nb + 1), per-warp counts (kBucketWarps x nb), indices (R)
+  // the RoI buckets live in stream-ordered scratch: reach rectangles (R float4), offsets (nb + 1), per-warp counts
+  // (kBucketWarps x nb), indices (R)
   const int nb = L.num_images * L.num_levels;
-  int* off = nullptr;
-  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&off), ((size_t)(kBucketWarps + 1) * nb + 1 + R) * sizeof(int), st);
+  float4* reach = nullptr;
+  cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&reach),
+                                  (size_t)R * sizeof(float4) + ((size_t)(kBucketWarps + 1) * nb + 1 + R) * sizeof(int), st);
   if (e != cudaSuccess) return set_error(C3D_ECUDA, "roi_align bwd buckets: %s", cudaGetErrorString(e));
+  int* off = reinterpret_cast<int*>(reach + R);
   int* wk = off + nb + 1;
   int* idx = wk + (size_t)kBucketWarps * nb;
-  roi_bucket_kernel<<<1, kBucketThreads, 0, st>>>(L, rois, R, nb, wk, off, idx);
+  roi_bucket_kernel<<<1, kBucketThreads, 0, st>>>(L, rois, R, nb, PH, PW, wk, off, idx, reach);
   int32_t rc = check_launch("roi_align bwd buckets");
   if (rc == C3D_OK) {
-    int bands = 0;
-    for (int i = 0; i < L.num_levels; ++i) bands += (L.H[i] + kTile - 1) / kTile;
-    roi_align_bwd_kernel<<<dim3((unsigned)bands, (unsigned)L.num_images), kTileC, sizeof(BwdSmem), st>>>(
-        L, rois, off, idx, C, PH, PW, (const bf16*)dout);
+    int tiles = 0;
+    for (int i = 0; i < L.num_levels; ++i) tiles += ((L.H[i] + kTile - 1) / kTile) * ((L.W[i] + kTile - 1) / kTile);
+    kernel<<<dim3((unsigned)tiles, (unsigned)L.num_images), kTileC, sizeof(BwdSmem), st>>>(L, rois, off, idx, reach, C, PH,
+                                                                                          PW, (const bf16*)dout);
     rc = check_launch("roi_align bwd");
   }
-  e = cudaFreeAsync(off, st);
+  e = cudaFreeAsync(reach, st);
   if (rc == C3D_OK && e != cudaSuccess) rc = set_error(C3D_ECUDA, "roi_align bwd buckets free: %s", cudaGetErrorString(e));
   return rc;
 }

@@ -172,12 +172,16 @@ def roi_align_fwd(feats, strides, rois, pooled=7):
     return out
 
 
-def roi_align_bwd(feats, strides, rois, dout, pooled=7):
-    """-> list of fp32 gradient maps shaped like feats (the kernel writes every element)."""
+def roi_align_bwd(feats, strides, rois, dout, pooled=7, dtype=torch.float32):
+    """-> list of gradient maps shaped like feats, fp32 or bf16 (the kernel writes every element; a bf16 map is the fp32
+    map rounded once)."""
+    if dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"roi_align_bwd: dtype must be float32 or bfloat16, not {dtype}")
     L = _lib.lib()
     C = feats[0].shape[-1]
-    grads = [torch.empty(f.shape, device=f.device, dtype=torch.float32) for f in feats]
+    grads = [torch.empty(f.shape, device=f.device, dtype=dtype) for f in feats]
     lv = _levels(feats, strides, grads)
+    lv.grad_bf16 = int(dtype == torch.bfloat16)
     _lib.check(L.c3d_roi_align_bwd(ctypes.byref(lv), ptr(rois), rois.shape[0], C, pooled, pooled, ptr(dout), stream()))
     return grads
 

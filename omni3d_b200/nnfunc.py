@@ -493,8 +493,8 @@ class ROIAlign(torch.autograd.Function):
     def backward(ctx, dout):
         rois, *feats = ctx.saved_tensors
         strides, pooled = ctx.cfg
-        grads = Kx.roi_align_bwd(feats, strides, rois, dout.contiguous(), pooled)
-        return (None, None, None) + tuple(_deliver(s, g.to(torch.bfloat16)) for s, g in zip(ctx.sinks, grads))
+        grads = Kx.roi_align_bwd(feats, strides, rois, dout.contiguous(), pooled, dtype=torch.bfloat16)
+        return (None, None, None) + tuple(_deliver(s, g) for s, g in zip(ctx.sinks, grads))
 
 
 class CubeLossRows(torch.autograd.Function):
