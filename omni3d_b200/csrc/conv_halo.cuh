@@ -385,6 +385,10 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------
+// halo_tensormap always describes dense images (H*W pixels apart): a different x_img_stride only matters between images
+static bool halo_dense_images(const c3d_conv_desc* d) {
+  return d->N <= 1 || d->x_img_stride == 0 || d->x_img_stride == (long long)d->H * d->W;
+}
 // pure function of the descriptor (c3d_conv2d_tiles must agree with c3d_conv2d_fwd)
 static bool halo_fwd_eligible(const c3d_conv_desc* d) {
   if (d->stride != 1 || d->KH != d->KW || !(d->KH & 1) || 2 * d->pad != d->KH - 1) return false;
@@ -392,7 +396,7 @@ static bool halo_fwd_eligible(const c3d_conv_desc* d) {
   if (!(d->Cin == 8 || d->Cin == 16 || d->Cin == 32)) return false;
   if (!(d->Cout == 16 || d->Cout == 32)) return false;
   if ((d->W < 128 && d->Cin != 8) || d->KH > 7) return false;   // NHWC8 input exists only for this kernel
-  return true;
+  return halo_dense_images(d) && d->y_split_c == 0;             // the GEMM kernels honour both fields
 }
 static bool halo_wgrad_eligible(const c3d_conv_desc* d) {
   if (d->stride != 1 || d->KH != d->KW || !(d->KH & 1) || 2 * d->pad != d->KH - 1) return false;
@@ -400,6 +404,7 @@ static bool halo_wgrad_eligible(const c3d_conv_desc* d) {
   if (!(d->Cout == 16 || d->Cout == 32)) return false;
   if (d->y_pix_stride != 0 && d->y_pix_stride != d->Cout) return false;
   if (d->W < 128 && d->Cin != 8) return false;
+  if (!halo_dense_images(d)) return false;
   return (d->KH == 7 && d->Cin == 8) || (d->KH == 3 && d->Cin >= 16);     // the compiled instances
 }
 // ring depth: the TMA rows are only 2-4 KB, so hiding ~1.5 us of L2/HBM latency at ~40 B/ns per SM needs tens of rows in flight
