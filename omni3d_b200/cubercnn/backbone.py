@@ -1,7 +1,7 @@
-"""DLA-34 / ResNet-34 bottom-up + FPN on the wgmma convolution kernels (NHWC bf16).
+"""DLA / torchvision ResNet bottom-ups + FPN on the wgmma convolution kernels (NHWC bf16).
 
 Mirrors the module tree, parameter names and initialisation order of
-cubercnn/modeling/backbone/dla.py:40-68,156-321,417-507 and resnet.py:12-96 (+ detectron2 FPN), so a
+cubercnn/modeling/backbone/dla.py:40-110,156-415,417-507 and resnet.py:12-96 (+ detectron2 FPN), so a
 reference checkpoint's state_dict loads unchanged and the same seed gives the same initial weights.  The
 nn.Conv2d / nn.BatchNorm2d modules below are PARAMETER HOLDERS (their forward is never called — every
 convolution / BatchNorm / pooling runs through omni3d_b200.nnfunc on libc3d.so).
@@ -76,33 +76,62 @@ class BasicBlock(nn.Module):
         return conv_bn(y, self.conv2, self.bn2, residual=residual)
 
 
+class Bottleneck(nn.Module):
+    """dla.py:71-109: 1x1 -> 3x3 (stride) -> 1x1 over planes // 2 channels, the residual added in the last conv's epilogue."""
+
+    def __init__(self, cin, cout, stride=1):
+        super().__init__()
+        mid = cout // 2
+        self.conv1 = nn.Conv2d(cin, mid, 1, bias=False)
+        self.bn1 = nn.BatchNorm2d(mid)
+        self.conv2 = nn.Conv2d(mid, mid, 3, stride=stride, padding=1, bias=False)
+        self.bn2 = nn.BatchNorm2d(mid)
+        self.conv3 = nn.Conv2d(mid, cout, 1, bias=False)
+        self.bn3 = nn.BatchNorm2d(cout)
+
+    def forward(self, x, residual=None):
+        if residual is None:
+            x, residual = fork(x, 2)
+        y = conv_bn(x, self.conv1, self.bn1)
+        y = conv_bn(y, self.conv2, self.bn2)
+        return conv_bn(y, self.conv3, self.bn3, residual=residual)
+
+
 class Root(nn.Module):
-    def __init__(self, cin, cout):
+    """dla.py:156-174; with `residual` (DLA-102 / 169) the first child is added before the ReLU."""
+
+    def __init__(self, cin, cout, residual=False):
         super().__init__()
         self.conv = nn.Conv2d(cin, cout, 1, bias=False)
         self.bn = nn.BatchNorm2d(cout)
+        self.residual = residual
 
     def forward(self, *xs):
+        res = None
+        if self.residual:
+            first, res = fork(xs[0], 2)
+            xs = (first,) + xs[1:]
         cat = CatChannels.apply(*xs) if torch.is_grad_enabled() else torch.cat(xs, dim=-1)
-        return conv_bn(cat, self.conv, self.bn)
+        return conv_bn(cat, self.conv, self.bn, residual=res)
 
 
 class Tree(nn.Module):
-    """dla.py:177-230.  For levels == 2 the outer `project` is dead weight in the reference (its output is
-    handed to an inner Tree that recomputes its own residual): parameters kept, never computed."""
+    """dla.py:177-230 for any `levels`.  A nested tree gets the stride and pools its own input.  For levels >= 2 the
+    `project` is dead weight in the reference (its output is handed to an inner Tree that recomputes its own residual):
+    parameters kept, never computed (omni3d_b200.train.unused_parameter_names)."""
 
-    def __init__(self, levels, cin, cout, stride=1, level_root=False, root_dim=0):
+    def __init__(self, levels, block, cin, cout, stride=1, level_root=False, root_dim=0, root_residual=False):
         super().__init__()
         root_dim = 2 * cout if root_dim == 0 else root_dim
         if level_root:
             root_dim += cin
         if levels == 1:
-            self.tree1 = BasicBlock(cin, cout, stride)
-            self.tree2 = BasicBlock(cout, cout, 1)
-            self.root = Root(root_dim, cout)
+            self.tree1 = block(cin, cout, stride)
+            self.tree2 = block(cout, cout, 1)
+            self.root = Root(root_dim, cout, root_residual)
         else:
-            self.tree1 = Tree(levels - 1, cin, cout, stride)
-            self.tree2 = Tree(levels - 1, cout, cout, root_dim=root_dim + cout)
+            self.tree1 = Tree(levels - 1, block, cin, cout, stride, root_residual=root_residual)
+            self.tree2 = Tree(levels - 1, block, cout, cout, root_dim=root_dim + cout, root_residual=root_residual)
         self.levels, self.level_root, self.stride = levels, level_root, stride
         self.project = None
         if cin != cout:
@@ -117,7 +146,7 @@ class Tree(nn.Module):
                 x, xp = fork(x, 2)
                 bottoms = list(fork(MaxPool2.apply(xp), n_bottom))
             else:
-                bottoms = []                     # (levels == 2 without level_root: the pooled map is never used)
+                bottoms = []                     # (levels >= 2 without level_root: the pooled map is never used)
         else:
             x, *bottoms = fork(x, 1 + n_bottom)
         if self.level_root:
@@ -134,16 +163,27 @@ class Tree(nn.Module):
         return self.tree2(x1a, children=children)
 
 
-class DLA34(nn.Module):
-    CH = [16, 32, 64, 128, 256, 512]
-    out_channels = {"p2": 64, "p3": 128, "p4": 256, "p5": 512, "p6": 512}
+# dla.py:312-415: levels of level2..level5, channels of base_layer..level5, block, root_residual.  level0 and level1 are one
+# 3x3 conv each in every type.  The DLA-X types need grouped 3x3 convolutions, which no kernel here computes.
+DLA_TYPES = {
+    "dla34": ((1, 2, 2, 1), (16, 32, 64, 128, 256, 512), BasicBlock, False),
+    "dla46_c": ((1, 2, 2, 1), (16, 32, 64, 64, 128, 256), Bottleneck, False),
+    "dla60": ((1, 2, 3, 1), (16, 32, 128, 256, 512, 1024), Bottleneck, False),
+    "dla102": ((1, 3, 4, 1), (16, 32, 128, 256, 512, 1024), Bottleneck, True),
+    "dla169": ((2, 3, 5, 1), (16, 32, 128, 256, 512, 1024), Bottleneck, True),
+}
+DLA_GROUPED_TYPES = ("dla46x_c", "dla60x_c", "dla60x", "dla102x", "dla102x2")
+
+
+class DLA(nn.Module):
     strides = {"p2": 4, "p3": 8, "p4": 16, "p5": 32, "p6": 64}
     # the 7x7 stride-1 stem runs on the rolling-halo kernel, which takes the image as NHWC8 (3 real channels)
     stem_cpad = 8
 
-    def __init__(self):
+    def __init__(self, dla_type="dla34"):
         super().__init__()
-        c = self.CH
+        levels, c, block, root_residual = DLA_TYPES[dla_type]
+        self.out_channels = {"p2": c[2], "p3": c[3], "p4": c[4], "p5": c[5], "p6": c[5]}      # dla.py:421-450
 
         def cbr(cin, cout, k, stride=1):
             return nn.Sequential(nn.Conv2d(cin, cout, k, stride=stride, padding=k // 2, bias=False),
@@ -151,10 +191,9 @@ class DLA34(nn.Module):
         self.base_layer = cbr(3, c[0], 7)
         self.level0 = cbr(c[0], c[0], 3)
         self.level1 = cbr(c[0], c[1], 3, stride=2)
-        self.level2 = Tree(1, c[1], c[2], 2, level_root=False)
-        self.level3 = Tree(2, c[2], c[3], 2, level_root=True)
-        self.level4 = Tree(2, c[3], c[4], 2, level_root=True)
-        self.level5 = Tree(1, c[4], c[5], 2, level_root=True)
+        for i in range(2, 6):
+            setattr(self, "level%d" % i, Tree(levels[i - 2], block, c[i - 1], c[i], 2, level_root=i > 2,
+                                              root_residual=root_residual))
         for m in self.modules():            # dla.py:262-268
             if isinstance(m, nn.Conv2d):
                 m.weight.data.normal_(0, math.sqrt(2.0 / (m.kernel_size[0] * m.kernel_size[1] * m.out_channels)))
@@ -173,18 +212,21 @@ class DLA34(nn.Module):
 
 
 class TVResNet(nn.Module):
-    """torchvision BasicBlock ResNet-18/34 topology (resnet.py:12-63); parameter names of torchvision."""
-    out_channels = DLA34.out_channels
-    strides = DLA34.strides
+    """torchvision ResNet-18/34 (BasicBlock) and ResNet-50/101 (Bottleneck) topologies (resnet.py:12-63); parameter names
+    and same-seed initialisation of torchvision."""
+    strides = DLA.strides
+    OUT_CHANNELS = {18: 64, 34: 64, 50: 256, 101: 256}          # p2 width; doubles per stage, p6 = p5 (resnet.py:16-27)
 
     def __init__(self, depth):
         super().__init__()
         from torchvision import models
-        if depth not in (18, 34):
-            raise ValueError("accelerated path covers the BasicBlock ResNets (BASELINE: ResNet34); got %d" % depth)
+        if depth not in self.OUT_CHANNELS:
+            raise ValueError("No configuration currently supporting depth of {}".format(depth))
         base = getattr(models, "resnet%d" % depth)(weights=None)
         for k in ("conv1", "bn1", "layer1", "layer2", "layer3", "layer4"):
             setattr(self, k, getattr(base, k))
+        c = self.OUT_CHANNELS[depth]
+        self.out_channels = {"p2": c, "p3": 2 * c, "p4": 4 * c, "p5": 8 * c, "p6": 8 * c}
 
     def forward(self, x):
         x = conv_bn(x, self.conv1, self.bn1)
@@ -196,7 +238,11 @@ class TVResNet(nn.Module):
                 if blk.downsample is not None:
                     idn = conv_bn(idn, blk.downsample[0], blk.downsample[1], relu=False)
                 y = conv_bn(x, blk.conv1, blk.bn1)
-                x = conv_bn(y, blk.conv2, blk.bn2, residual=idn)
+                if hasattr(blk, "conv3"):        # torchvision Bottleneck: 1x1, 3x3 carrying the stride, 1x1 + residual
+                    y = conv_bn(y, blk.conv2, blk.bn2)
+                    x = conv_bn(y, blk.conv3, blk.bn3, residual=idn)
+                else:
+                    x = conv_bn(y, blk.conv2, blk.bn2, residual=idn)
             x, out[name] = fork(x, 2)
         out["p6"] = x[:, ::2, ::2, :].contiguous()
         return out
@@ -253,11 +299,15 @@ def _check_weights(cfg):
 @BACKBONE_REGISTRY.register()
 def build_dla_from_vision_fpn_backbone(cfg, input_shape=None, priors=None):
     _check_weights(cfg)
-    if cfg.MODEL.DLA.TYPE != "dla34":
-        raise NotImplementedError("accelerated path covers dla34 (BASELINE configs); got " + cfg.MODEL.DLA.TYPE)
+    t = cfg.MODEL.DLA.TYPE
+    if t in DLA_GROUPED_TYPES:
+        raise NotImplementedError("MODEL.DLA.TYPE %s needs grouped 3x3 convolutions, which the accelerated path does not "
+                                  "compute; supported: %s" % (t, ", ".join(DLA_TYPES)))
+    if t not in DLA_TYPES:
+        raise NotImplementedError("unknown MODEL.DLA.TYPE %s; supported: %s" % (t, ", ".join(DLA_TYPES)))
     if cfg.MODEL.FPN.NORM != "" or cfg.MODEL.FPN.FUSE_TYPE != "sum":
         raise NotImplementedError("FPN NORM/FUSE_TYPE other than ''/'sum'")
-    return FPN(DLA34(), cfg.MODEL.FPN.IN_FEATURES, cfg.MODEL.FPN.OUT_CHANNELS)
+    return FPN(DLA(t), cfg.MODEL.FPN.IN_FEATURES, cfg.MODEL.FPN.OUT_CHANNELS)
 
 
 @BACKBONE_REGISTRY.register()

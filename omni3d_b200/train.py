@@ -33,17 +33,18 @@ def _world():
 
 
 def unused_parameter_names(model):
-    """Parameters the reference never reaches in forward (find_unused_parameters=True, train_net.py:451):
-    the outer `project` of the two-level DLA trees (dla.py:217-230) and the priors (detached, roi_heads.py:470)."""
+    """Parameters the reference never reaches in forward (find_unused_parameters=True, train_net.py:451): the priors
+    (detached, roi_heads.py:470) and every `project` that is not a one-level DLA tree's.  A tree with levels >= 2 hands
+    its projected residual to an inner tree that recomputes its own (dla.py:217-230), so only `levels == 1` computes it."""
     out = set()
     for name, _ in model.named_parameters():
-        parts = name.split(".")
         if "priors_dims_per_cat" in name or "priors_z_scales" in name:
             out.add(name)
-        if "project" in parts:
-            i = parts.index("project")
-            if parts[i - 1] in ("level3", "level4"):
-                out.add(name)
+    for mod_name, m in model.named_modules():
+        project = getattr(m, "project", None)
+        if isinstance(project, torch.nn.Module) and getattr(m, "levels", None) != 1:
+            prefix = (mod_name + "." if mod_name else "") + "project."
+            out.update(prefix + n for n, _ in project.named_parameters())
     return out
 
 
