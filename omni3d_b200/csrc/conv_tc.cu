@@ -294,14 +294,20 @@ struct WgradKParams {
   long long welems;
   int oihw;                                  // 0: dw is [Cout][KH][KW][Cin]; 1: [Cout][Cin][KH][KW] (master layout)
   int big, mc;                               // 1: 5-D tensor maps — ONE box carries all channel chunks of dY (and mc chunks of X)
+  int sub;                                   // row slices per pixel tile: each slice of RH / sub rows is one ring slot
+  int slots, slot_bytes, b_off;              // kStages * sub slots of kStageBytes / sub bytes; x boxes at b_off in a slot
   int lin;                                   // 1: fully-connected layer (c3d_linear_wgrad): x is (rows, KH*KW*Cin) with the
                                              // features in (tap, ci) order — box b reads channels [b*cw, (b+1)*cw) with no
                                              // spatial shift; KH/KW/Cin only drive the epilogue's master-layout index
 };
 
-// two pipeline stages of kPix pixels (GEMM K) x up to kCols GEMM columns per CTA (192 KB)
+// kStages pixel tiles of up to kPix pixels (GEMM K) x up to kCols GEMM columns per CTA (192 KB).  A tile whose rows
+// divide is loaded and consumed as `sub` <= kMaxSlices row slices, each a ring slot of its own (kStages * sub slots of
+// kStageBytes / sub bytes): the same bytes are in flight, but a slot is refilled as soon as ITS 128 / sub pixels have been
+// multiplied, so several loads overlap one slice's MMAs instead of one load overlapping one tile's.  The MMAs run over the
+// same pixels in the same order, so the sums are bit-identical to whole-tile stages.
 struct WgradSmem {
-  static constexpr int kStages = 2, kPix = 128, kCols = 256;
+  static constexpr int kStages = 2, kPix = 128, kCols = 256, kMaxSlices = 2;
   static constexpr int kABytes = kPix * 128 * 2;           // up to two [kPix px][64 ch] chunks (or narrower)
   static constexpr int kBBytes = kPix * kCols * 2;         // kCols columns x kPix pixels
   static constexpr int kStageBytes = kABytes + kBBytes;    // 96 KB
@@ -323,19 +329,19 @@ __device__ __forceinline__ void wgrad_consume(const WgradKParams& P, uint8_t* sm
 #pragma unroll
   for (int i = 0; i < NB / 2; ++i) acc[i] = 0.f;
   const uint32_t lt_a = ptx::swizzle_layout_type(P.ca * 2), lt_b = ptx::swizzle_layout_type(P.cw * 2);
-  const int ksteps = (P.RH * P.RW) / 16;
+  const int ksteps = (P.RH * P.RW) / (16 * P.sub);
   // MN-major descriptors: LBO = distance between channel chunks, SBO = 8 pixel rows
   const uint32_t a_sbo = 8 * P.ca * 2, b_sbo = 8 * P.cw * 2;
   const uint32_t a_kstep = (16 * P.ca * 2) >> 4, b_kstep = (16 * P.cw * 2) >> 4;
   const uint32_t a_off = (uint32_t)(wg * (64 / P.ca)) * a_box_bytes;   // first dY chunk of this warpgroup's channels
   int stage = 0; uint32_t phase = 0;
   int prev = -1;
-  for (int t = t_begin; t < t_end; ++t) {
+  for (int t = (t_end - t_begin) * P.sub; t > 0; --t) {
     ptx::mbar_wait(&full_bar[stage], phase);
     if (active) {
-      const uint32_t sa = ptx::smem_u32(smem + stage * S::kStageBytes);
+      const uint32_t sa = ptx::smem_u32(smem) + stage * P.slot_bytes;
       const uint64_t da = ptx::make_smem_desc(sa + a_off, a_box_bytes, a_sbo, lt_a);
-      const uint64_t db = ptx::make_smem_desc(sa + S::kABytes, b_box_bytes, b_sbo, lt_b);
+      const uint64_t db = ptx::make_smem_desc(sa + P.b_off, b_box_bytes, b_sbo, lt_b);
       ptx::wgmma_fence();
       for (int k = 0; k < ksteps; ++k)
         ptx::wgmma_bf16<NB, 1, 1>(acc, da + (uint64_t)(a_kstep * k), db + (uint64_t)(b_kstep * k), 1u);
@@ -344,7 +350,7 @@ __device__ __forceinline__ void wgrad_consume(const WgradKParams& P, uint8_t* sm
     }
     if (prev >= 0) { __syncwarp(); if (lane == 0) ptx::mbar_arrive(&empty_bar[prev]); }
     prev = stage;
-    if (++stage == S::kStages) { stage = 0; phase ^= 1; }
+    if (++stage == P.slots) { stage = 0; phase ^= 1; }
   }
   ptx::wgmma_wait<0>();
   ptx::fence_regs(acc);
@@ -413,7 +419,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
-  uint64_t* empty_bar = full_bar + S::kStages;
+  uint64_t* empty_bar = full_bar + S::kStages * S::kMaxSlices;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   const int split = blockIdx.x, group = blockIdx.y, co_tile = blockIdx.z;
@@ -424,15 +430,16 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
   const int t_begin = split * P.tiles_per_split;
   const int t_end = min(P.num_tiles, t_begin + P.tiles_per_split);
   if (t_begin >= t_end) return;
-  const int R = P.RH * P.RW;
+  const int RHs = P.RH / P.sub, R = RHs * P.RW;                   // rows and pixels of one slice
   int a_chunks = (P.Cout - co0 + P.ca - 1) / P.ca;
   if (a_chunks > P.a_chunks_max) a_chunks = P.a_chunks_max;
-  // distance between channel chunks in shared memory: a full kPix-pixel slot per box, or (5-D boxes) the dense box pitch
-  const uint32_t a_box_bytes = (uint32_t)((P.big ? R : S::kPix) * P.ca * 2), b_box_bytes = (uint32_t)((P.big ? R : S::kPix) * P.cw * 2);
+  // distance between channel chunks in shared memory: a full kPix / sub-pixel slot per box, or (5-D boxes) the dense box pitch
+  const int pitch_pix = P.big ? R : S::kPix / P.sub;
+  const uint32_t a_box_bytes = (uint32_t)(pitch_pix * P.ca * 2), b_box_bytes = (uint32_t)(pitch_pix * P.cw * 2);
 
   if (warp == kConsumerWarps && lane == 0) {
     ptx::prefetch_tensormap(&tmap_dy); ptx::prefetch_tensormap(&tmap_x);
-    for (int s = 0; s < S::kStages; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kConsumerWarps); }
+    for (int s = 0; s < P.slots; ++s) { ptx::mbar_init(&full_bar[s], 1); ptx::mbar_init(&empty_bar[s], kConsumerWarps); }
     ptx::fence_barrier_init();
   }
   __syncthreads();
@@ -441,12 +448,13 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
     if (ptx::elect_one()) {
       int stage = 0; uint32_t phase = 0;
       const uint32_t bytes = (uint32_t)(R * 2 * ((P.big ? P.a_chunks_max : a_chunks) * P.ca + nb * P.cw));
-      for (int t = t_begin; t < t_end; ++t) {
+      for (int ts = t_begin * P.sub; ts < t_end * P.sub; ++ts) {
+        const int t = ts / P.sub;
         const int tw_i = t % P.tiles_w, th_i = (t / P.tiles_w) % P.tiles_h, img = t / (P.tiles_w * P.tiles_h);
-        const int ho0 = th_i * P.RH, wo0 = tw_i * P.RW;
+        const int ho0 = th_i * P.RH + (ts - t * P.sub) * RHs, wo0 = tw_i * P.RW;
         ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * S::kStageBytes;
-        uint8_t* sb = sa + S::kABytes;
+        uint8_t* sa = smem + stage * P.slot_bytes;
+        uint8_t* sb = sa + P.b_off;
         ptx::mbar_expect_tx(&full_bar[stage], bytes);
         if (P.big) {
           ptx::tma_load_5d(sa, &tmap_dy, &full_bar[stage], 0, wo0, ho0, co0 / P.ca, img);
@@ -474,7 +482,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
                                wo0 * P.stride + kw - P.pad, ho0 * P.stride + kh - P.pad, img);
           }
         }
-        if (++stage == S::kStages) { stage = 0; phase ^= 1; }
+        if (++stage == P.slots) { stage = 0; phase ^= 1; }
       }
     }
   } else {
@@ -641,6 +649,9 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
     P.Cin = lin_c; P.KH = lin_pp; P.KW = 1;      // epilogue index space: (tap = p, ci = c); the loader ignores kh / kw
   }
   pick_tile_k(Ho, Wo, d->stride, &P.RH, &P.RW);
+  P.sub = WgradSmem::kMaxSlices;                 // the most row slices of whole 16-pixel MMA steps
+  while (P.sub > 1 && (P.RH % P.sub != 0 || (P.RH / P.sub * P.RW) % 16 != 0)) P.sub >>= 1;
+  P.slots = WgradSmem::kStages * P.sub; P.slot_bytes = WgradSmem::kStageBytes / P.sub; P.b_off = WgradSmem::kABytes / P.sub;
   P.tiles_h = (Ho + P.RH - 1) / P.RH; P.tiles_w = (Wo + P.RW - 1) / P.RW;
   P.num_tiles = d->N * P.tiles_h * P.tiles_w;
   const int taps = P.KH * P.KW;
@@ -679,11 +690,11 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
     const long long ximg = d->x_img_stride ? d->x_img_stride : (long long)d->W * d->H;
     cuuint64_t dy_dims[5] = {(cuuint64_t)P.ca, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)nca, (cuuint64_t)d->N};
     cuuint64_t dy_str[4] = {(cuuint64_t)yps * 2, (cuuint64_t)yps * 2 * Wo, (cuuint64_t)P.ca * 2, (cuuint64_t)yps * 2 * Wo * Ho};
-    cuuint32_t dy_box[5] = {(cuuint32_t)P.ca, (cuuint32_t)P.RW, (cuuint32_t)P.RH, (cuuint32_t)P.a_chunks_max, 1};
+    cuuint32_t dy_box[5] = {(cuuint32_t)P.ca, (cuuint32_t)P.RW, (cuuint32_t)(P.RH / P.sub), (cuuint32_t)P.a_chunks_max, 1};
     cuuint32_t one5[5] = {1, 1, 1, 1, 1};
     cuuint64_t x_dims[5] = {(cuuint64_t)P.cw, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)nchunks_x, (cuuint64_t)d->N};
     cuuint64_t x_str[4] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cin * 2 * d->W, (cuuint64_t)P.cw * 2, (cuuint64_t)Cin * 2 * ximg};
-    cuuint32_t x_box[5] = {(cuuint32_t)P.cw, (cuuint32_t)(P.RW * d->stride), (cuuint32_t)(P.RH * d->stride), (cuuint32_t)mc, 1};
+    cuuint32_t x_box[5] = {(cuuint32_t)P.cw, (cuuint32_t)(P.RW * d->stride), (cuuint32_t)(P.RH / P.sub * d->stride), (cuuint32_t)mc, 1};
     cuuint32_t x_es[5] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1, 1};
     CUresult r1 = enc(&mdy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(dy), dy_dims, dy_str, dy_box, one5,
                       CU_TENSOR_MAP_INTERLEAVE_NONE, swz(P.ca * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -701,7 +712,7 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)d->N};
     cuuint64_t strides[3] = {(cuuint64_t)yps * 2, (cuuint64_t)yps * 2 * Wo, (cuuint64_t)yps * 2 * Wo * Ho};
-    cuuint32_t box[4] = {(cuuint32_t)P.ca, (cuuint32_t)P.RW, (cuuint32_t)P.RH, 1};
+    cuuint32_t box[4] = {(cuuint32_t)P.ca, (cuuint32_t)P.RW, (cuuint32_t)(P.RH / P.sub), 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = enc(&mdy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(dy), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, swz(P.ca * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -712,7 +723,7 @@ static int32_t wgrad_impl(const c3d_conv_desc* d, const void* x, const void* dy,
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->N};
     cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cin * 2 * d->W,
                              (cuuint64_t)Cin * 2 * (d->x_img_stride ? d->x_img_stride : (long long)d->W * d->H)};
-    cuuint32_t box[4] = {(cuuint32_t)P.cw, (cuuint32_t)(P.RW * d->stride), (cuuint32_t)(P.RH * d->stride), 1};
+    cuuint32_t box[4] = {(cuuint32_t)P.cw, (cuuint32_t)(P.RW * d->stride), (cuuint32_t)(P.RH / P.sub * d->stride), 1};
     cuuint32_t estr[4] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1};
     CUresult r = enc(&mx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, swz(P.cw * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
